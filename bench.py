@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the TA3N hot path on B200 (metric of BASELINE.json).
+"""bench.py -- throughput of the TA3N hot path on an H100 (metric of BASELINE.json).
 
     python bench.py --gpus N --steps K --warmup W            # this repo (CUDA path through the C ABI)
     python bench.py --impl reference --gpus N --steps K ...  # the unmodified reference on the host cores, rank 0
@@ -10,7 +10,8 @@ VideoModel.forward (train mode, dropout 0.5/0.5), the composed loss of the shipp
 parameter gradients (+ the gradient all-reduce when N > 1).  clips per step = 2B per GPU.
 The optimizer is outside the metric (BASELINE.json: "fwd+bwd"); the e2e leg includes it.
 
-Prints ONE JSON line on rank 0 (schema: see the task contract).
+Prints ONE JSON line on rank 0.  --dump-outputs DIR also writes what the last timed step computed (its loss and
+every parameter gradient) as DIR/<name>.npy, so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -48,7 +49,12 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="enqueue the step eagerly instead of replaying a CUDA graph")
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="CPU budget of the cpu_baseline sample")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the loss and parameter gradients of the last timed step as DIR/<name>.npy (float32)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 # ------------------------------------------------------------------------------------------------
@@ -93,7 +99,7 @@ def traffic_model(M, T, F, C):
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -145,7 +151,7 @@ def measured_peaks():
         with open(path) as f:
             p = json.load(f)
         return float(p["hbm_gbs"]), float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 0))), "measured"
-    return 6650.0, 1590.0, "fallback"        # B200_PROFILING.md fallback
+    return 3350.0, 989.0, "datasheet"        # H100 SXM data sheet: HBM3 GB/s, dense BF16 TFLOP/s (700 W card)
 
 
 def pick_engine(requested):
@@ -312,6 +318,29 @@ def workload_config(args, world, engine):
                       "device-side spin so host launch gaps are outside the events"}
 
 
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, model, step, loss):
+    """The loss and every parameter gradient of the step just run, as <name>.npy (float32).  When they exceed
+    DUMP_BUDGET_BYTES together, each array larger than its equal share of the budget is replaced by a fixed, seeded
+    sample of that many elements, <name>.sample.npy (flat), so that two builds still compare element for element."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    names = {id(p): n for n, p in model.named_parameters()}
+    arrays = {"loss": loss}
+    arrays.update({"grad." + names[id(p)]: g for p, g in zip(step.params, step.grad_views) if g is not None})
+    total = sum(t.numel() for t in arrays.values()) * 4
+    share = DUMP_BUDGET_BYTES // 4 // len(arrays)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if total > DUMP_BUDGET_BYTES and a.size > share:
+            idx = np.sort(np.random.default_rng(1234).choice(a.size, share, replace=False))
+            np.save(os.path.join(out_dir, name + ".sample.npy"), a.reshape(-1)[idx])
+        else:
+            np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 # ------------------------------------------------------------------------------------------------
 def run_b200(args):
     import torch
@@ -374,9 +403,11 @@ def run_b200(args):
     for k in range(args.steps):
         flush.fill_(k & 0xFF)
         ev[k][0].record()
-        step.run()
+        last_loss = step.run()
         ev[k][1].record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, step, last_loss)
     launches = step.launches_per_step * args.steps
     t_ms = sum(a.elapsed_time(b) for a, b in ev)
     t = torch.tensor([t_ms], device=dev, dtype=torch.float64)
@@ -495,17 +526,8 @@ def run_b200(args):
         cnt, ms = rep[dom]
         per_step_ms = ms / n_prof                      # all launches of this call site in one step
         ach = tm["sites"][dom] / (per_step_ms * 1e-3) / 1e9
-        traffic = None
-        try:   # DRAM bytes of this call site from the committed `ncu --set full` capture (profiles/)
-            with open(os.path.join(ROOT, "profiles", "r2_traffic.json")) as f:
-                traffic = json.load(f)["dram_bytes_per_step"].get(dom) if (B, T, F, C) == (256, 5, 512, 12) else None
-        except Exception:
-            pass
         roof = {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
-                "frac": ach / hbm_peak, "traffic": traffic,
-                "traffic_source": "profiles/r2_step_full.txt (ncu --set full of one step of this binary, tf32x3 engine: "
-                                  "dram__bytes_read+write of the launch)",
-                "peak_kind": peak_kind,
+                "frac": ach / hbm_peak, "peak_kind": peak_kind,
                 "algorithmic_bytes_per_step": tm["sites"][dom], "kernel_ms_per_step": per_step_ms,
                 "share_of_library_time": ms / total_site_ms, "launches_per_step": cnt / n_prof}
     ach_b = tm["scope_b"] / (step_ms * 1e-3) / 1e9

@@ -1,5 +1,5 @@
 /*
- * ta3n_b200.h -- C ABI of libta3n_sm100.so: the B200 (sm_100a) implementation of the
+ * ta3n_b200.h -- C ABI of libta3n_sm90.so: the H100 (sm_90a) implementation of the
  * TA3N hot path (TRN-M relation aggregation + domain-attentive pooling + gradient-reversal
  * discriminators inside VideoModel.forward of cmhungsteve/TA3N).
  *
@@ -45,7 +45,7 @@ enum {
 /* GEMM engines for the dense contractions. */
 enum {
   TA3N_GEMM_FP32_SIMT = 0,   /* exact fp32 FFMA tiles (parity / debugging engine)     */
-  TA3N_GEMM_TF32_TCGEN05 = 1,/* tcgen05.mma kind::tf32, TMA-staged, TMEM accumulators: fastest, forward ~3e-4      */
+  TA3N_GEMM_TF32_TCGEN05 = 1,/* wgmma tf32, TMA-staged, register accumulators: fastest, forward ~3e-4      */
   TA3N_GEMM_TF32X3_TCGEN05 = 2 /* the default: the same engine with every FORWARD layer at fp32 grade (operands split
                                   in two tf32 pieces, three products per K step, K accumulated in chunks of 256), so that
                                   no ReLU unit changes state against the fp32 reference; backward GEMMs as engine 1  */

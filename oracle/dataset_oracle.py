@@ -8,6 +8,7 @@ running the reference itself.  Only tests may import this module.
 """
 from __future__ import annotations
 
+import os
 from typing import List
 
 import numpy as np
@@ -76,3 +77,22 @@ def repeat_list(n_items: int, num_dataload: int) -> List[int]:
     n_repeat, n_left = num_dataload // n_items, num_dataload % n_items
     base = list(range(n_items))
     return base * n_repeat + base[:n_left]
+
+
+def make_feature_tree(root, n_videos=7, feat_dim=16, seed=3):
+    """A miniature dataset in the reference's on-disk format: <root>/vK/img_00001.t7 ... one tensor per frame."""
+    import torch
+
+    g = torch.Generator().manual_seed(seed)
+    lines = []
+    for v in range(n_videos):
+        nf = int(torch.randint(2, 14, (1,), generator=g))
+        d = os.path.join(root, f"v{v}")
+        os.makedirs(d)
+        for f in range(1, nf + 1):
+            torch.save(torch.randn(feat_dim, generator=g), os.path.join(d, "img_{:05d}.t7".format(f)))
+        lines.append(f"{d} {nf} {v % 3}")
+    lst = os.path.join(root, "list.txt")
+    with open(lst, "w") as fh:
+        fh.write("\n".join(lines) + "\n")
+    return lst

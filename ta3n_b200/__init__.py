@@ -1,4 +1,4 @@
-"""ta3n_b200 -- B200 (sm_100a) implementation of the TA3N hot path.
+"""ta3n_b200 -- H100 (sm_90a) implementation of the TA3N hot path.
 
 Drop-in for the reference's ``models.VideoModel`` / ``TRNmodule.RelationModuleMultiScale`` /
 ``opts.parser`` on the path ``frame_aggregation='trn-m'`` (TRN-M relation aggregation +

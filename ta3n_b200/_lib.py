@@ -1,4 +1,4 @@
-"""ctypes binding of libta3n_sm100.so (the C ABI in include/ta3n_b200.h).
+"""ctypes binding of libta3n_sm90.so (the C ABI in include/ta3n_b200.h).
 
 There is no CPU fallback: if the shared library is missing this module raises, and every
 wrapper refuses tensors that are not CUDA fp32 contiguous.
@@ -149,7 +149,7 @@ def load() -> C.CDLL:
                 fn.restype = res
                 fn.argtypes = args
             if lib.ta3n_abi_version() != 2:
-                raise Ta3nError("libta3n_sm100.so ABI version mismatch")
+                raise Ta3nError("libta3n_sm90.so ABI version mismatch")
             _lib = lib
     return _lib
 
@@ -157,7 +157,7 @@ def load() -> C.CDLL:
 def check(rc: int) -> None:
     if rc != 0:
         msg = load().ta3n_last_error()
-        raise Ta3nError(f"libta3n_sm100 error {rc}: {msg.decode() if msg else '?'}")
+        raise Ta3nError(f"libta3n_sm90 error {rc}: {msg.decode() if msg else '?'}")
 
 
 def ptr_array(ptrs):
@@ -166,7 +166,7 @@ def ptr_array(ptrs):
 
 
 def set_gemm_engine(engine) -> None:
-    """'tf32x3' (tcgen05, error-compensated tf32: fp32-grade forward; the library default), 'tf32' (plain tcgen05
+    """'tf32x3' (wgmma, error-compensated tf32: fp32-grade forward; the library default), 'tf32' (plain wgmma
     tf32) or 'fp32' (exact SIMT tiles)."""
     code = {"fp32": TA3N_GEMM_FP32_SIMT, "tf32": TA3N_GEMM_TF32_TCGEN05, "tf32x3": TA3N_GEMM_TF32X3_TCGEN05}.get(engine, engine)
     check(load().ta3n_set_gemm_engine(int(code)))
@@ -176,7 +176,7 @@ def get_gemm_engine() -> str:
     return {0: "fp32", 1: "tf32", 2: "tf32x3"}[load().ta3n_get_gemm_engine()]
 
 
-def plan_forward_splits(shapes, sms: int = 148, scratch_bytes: int = 48 << 20):
+def plan_forward_splits(shapes, sms: int = 132, scratch_bytes: int = 48 << 20):
     """Split-K factors the tf32x3 engine's balanced planner picks for one forward launch of GEMMs [(M, N, K), ...]
     (host-only, C ABI ta3n_plan_forward_splits).  Returns (ksplit list, unsplit makespan, chosen makespan)."""
     n = len(shapes)

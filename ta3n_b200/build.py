@@ -1,4 +1,4 @@
-"""Build recipe for libta3n_sm100.so (nvcc, sm_100a only; cross-compiles without a GPU)."""
+"""Build recipe for libta3n_sm90.so (nvcc, sm_90a only; cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -8,13 +8,13 @@ import sys
 
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
-LIB_PATH = os.path.join(PKG_DIR, "libta3n_sm100.so")
+LIB_PATH = os.path.join(PKG_DIR, "libta3n_sm90.so")
 SOURCES = ["ta3n_api.cu"]
-HEADERS = ["common.cuh", "seg_gemm.cuh", "rowops.cuh", "gemm_tcgen05.cuh", "optim.cuh", "step_rows.cuh",
+HEADERS = ["common.cuh", "seg_gemm.cuh", "rowops.cuh", "gemm_wgmma.cuh", "optim.cuh", "step_rows.cuh",
            "step_kernel.cuh", "step_plan.cuh", "allreduce.cuh",
            os.path.join("..", "..", "include", "ta3n_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 
@@ -23,7 +23,7 @@ def _nvcc() -> str:
     for cand in (shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found; cannot build libta3n_sm100.so")
+    raise RuntimeError("nvcc not found; cannot build libta3n_sm90.so")
 
 
 def needs_build() -> bool:

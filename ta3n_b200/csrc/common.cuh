@@ -1,5 +1,5 @@
 // common.cuh -- error plumbing, launch accounting and small device helpers shared by every
-// translation unit of libta3n_sm100.so.
+// translation unit of libta3n_sm90.so.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -127,7 +127,7 @@ inline std::atomic<int>& gemm_engine() {
 // Every kernel starts with pdl_wait() (griddepcontrol.wait: the previous kernel in the stream has completed
 // and its writes are visible) after whatever set-up needs no device data, then allows ITS dependents to be
 // scheduled.  With the launch attribute below, kernel k+1's CTAs are placed on idle SMs and run their
-// prologue (parameter staging, barrier init, TMEM allocation) while kernel k is still computing -- the
+// prologue (parameter staging, barrier init) while kernel k is still computing -- the
 // step is a chain of ~26 short, mostly sub-wave kernels, so launch latency and prologues are on the
 // critical path.  TA3N_PDL=0 disables the attribute (the device-side instructions are then no-ops).
 inline bool pdl_enabled() {

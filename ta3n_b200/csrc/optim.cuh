@@ -13,7 +13,7 @@
 
 namespace ta3n {
 
-constexpr int kSqnormBlocks = 296;     // 2 per SM on a 148-SM part; also the number of partials
+constexpr int kSqnormBlocks = 296;     // 2+ per SM on a 132-SM part; also the number of partials
 constexpr int kOptThreads = 256;
 
 __device__ __forceinline__ float block_sum_256(float s, float* red) {

@@ -25,7 +25,7 @@ struct RelMap {
 
 inline unsigned blocks_for(size_t n, int threads) {
   size_t b = (n + threads - 1) / threads;
-  if (b > 148u * 32u) b = 148u * 32u;   // grid-stride beyond 32 CTAs per SM
+  if (b > 132u * 32u) b = 132u * 32u;   // grid-stride beyond 32 CTAs per SM
   if (b == 0) b = 1;
   return (unsigned)b;
 }
@@ -215,7 +215,7 @@ inline int launch_head_fwd(const float* x, int ldx, const float* W, const float*
   const size_t wbytes = (size_t)N2 * K * sizeof(float);
   const int in_smem = wbytes <= 48 * 1024 ? 1 : 0;
   size_t blocks = ((size_t)rows + 3) / 4;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (blocks == 0) blocks = 1;
   pre_launch("head_fwd", st);
   launch_kernel(head_fwd_kernel, (unsigned)blocks, 128, in_smem ? wbytes : 0, st, x, ldx, W, b, out, ldo, rows, K, N2, in_smem, d, x_out);

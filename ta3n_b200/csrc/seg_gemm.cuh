@@ -14,7 +14,7 @@
 //   B_KMAJ: B(k,n) = B[n*ldb + k]   (nn.Linear weight, forward)    else B(k,n) = B[k*ldb + n]
 //
 // This file holds the table types, the epilogue, the exact-fp32 SIMT engine and the split-K
-// reducer.  The tcgen05 engine (gemm_tcgen05.cuh) consumes the same tables.
+// reducer.  The tensor-core engine (gemm_wgmma.cuh) consumes the same tables.
 #pragma once
 
 #include <vector>
@@ -106,7 +106,7 @@ inline Group make_group() {
   return g;
 }
 
-// ---- epilogue (shared by the SIMT engine, the split-K reducer and the tcgen05 engine) --------
+// ---- epilogue (shared by the SIMT engine, the split-K reducer and the tensor-core engine) --------
 // F >= 0: flag set known at compile time (dead branches -- notably the 64-bit RNG mixing -- vanish);
 // F < 0 : generic, flags read at run time.  The kernels dispatch the common sets to the specialised
 // instantiations: evaluated per output element, the generic form costs ~100 issued instructions even when
@@ -190,7 +190,7 @@ __device__ __forceinline__ void drop_row32(const Group& g, const int f, int m, i
   }
 }
 
-// The same epilogue applied to a 32-column segment (m, nb..nb+31) held by one thread (tcgen05 engine: one
+// The same epilogue applied to a 32-column segment (m, nb..nb+31) held by one thread (tensor-core engine: one
 // accumulator row per lane).  Auxiliary operands (bias, add, gate, C) are fetched as whole 128 B row pieces
 // with vector loads up front instead of one dependent scalar load per element.
 // generic form (flags read at run time; rare flag sets only): one auxiliary row at a time, few registers
@@ -343,7 +343,7 @@ struct SegLite {
   const float* A;
   const float* B;
   int len, lda, ldb;
-  unsigned short amap, bmap;   // tensor-map slots (tcgen05 engine only)
+  unsigned short amap, bmap;   // tensor-map slots (tensor-core engine only)
 };
 constexpr int kCtxMaxSegs = kMaxSegs;
 
@@ -658,7 +658,7 @@ struct GemmPlan {
   std::vector<Seg> segs;     // group.seg_begin indexes into this vector
   bool a_kmaj = true, b_kmaj = true;
   int load_flags = 0;
-  bool precise = false;             // a forward layer: the x3 engine runs it at fp32 grade (gemm_tcgen05.cuh)
+  bool precise = false;             // a forward layer: the x3 engine runs it at fp32 grade (gemm_wgmma.cuh)
   bool precise_dgrad = false;       // a data-gradient GEMM (feeds further GEMMs): x3 engine, fp32 grade as well
   const char* label = "seg_gemm";   // call-site name used by the timing registry
 
@@ -695,7 +695,7 @@ struct GemmPlan {
 // Choose a split-K factor for reduction-heavy, tile-poor problems (wgrads) and carve the partial
 // buffers out of `arena` (which may be null -> no split-K).  bm/bn/bk: tile shape of the engine.
 inline void plan_splitk(GemmPlan& plan, Arena* arena, int bm, int bn, int bk, int min_chunks,
-                        int target_ctas = 148) {
+                        int target_ctas = 132) {
   if (!arena) return;
   long tiles = 0;
   for (auto& g : plan.groups) tiles += (long)((g.M + bm - 1) / bm) * ((g.N + bn - 1) / bn);

@@ -1,10 +1,10 @@
 // step_kernel.cuh -- the fused training step of the path as ONE persistent kernel.
 //
 // main.py:418-576 for the shipped configuration (forward of VideoModel.forward models.py:545-722, the composed loss,
-// backward to every parameter gradient) is a static graph of ~900 small tasks: 128x128 tcgen05 GEMM tiles
-// (gemm_tcgen05.cuh::tc_tile), per-video row tasks and column-sum tasks (step_rows.cuh).  Run as separate launches
-// (round 1: 25 kernels, every one sub-wave) the step is the SUM of per-launch critical paths plus a drain and a
-// pipeline fill at every kernel boundary: 0.27 ms for 20 us of HBM traffic.  Here one CTA per SM pulls tasks from
+// backward to every parameter gradient) is a static graph of ~900 small tasks: 128x128 wgmma GEMM tiles
+// (gemm_wgmma.cuh), per-video row tasks and column-sum tasks (step_rows.cuh).  Run as separate launches
+// (25 kernels, every one sub-wave) the step is the SUM of per-launch critical paths plus a drain and a
+// pipeline fill at every kernel boundary.  Here one CTA per SM pulls tasks from
 // priority queues; a task becomes eligible when the arrival counters of the tasks that produce its inputs have reached
 // their targets (release / acquire through global memory), so
 //   * dependent stages overlap at 128-row granularity instead of at kernel boundaries,
@@ -23,18 +23,21 @@
 // summation order -> bit-identical reruns.
 #pragma once
 
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include "step_rows.cuh"
 
 namespace ta3n {
 
-constexpr int kStepThreads = 352;     // warp 0 TMA producer, 1 MMA issuer, 2..9 epilogue / row tasks, 10 scheduler
-constexpr int kStepStages = 5;        // operand ring: 5 x 32 KB
+// warps 0..7: the two wgmma consumer warpgroups of the GEMM tiles, the epilogue and the row tasks; 8 TMA producer;
+// 9 scheduler
+constexpr int kStepThreads = 320;
+constexpr int kStepProducerWarp = 8, kStepSchedulerWarp = 9;
+constexpr int kStepStages = 3;        // operand ring: 3 x 32 KB
 constexpr int kStepSlots = 3;         // tasks a CTA holds at once (scheduled ahead of the one being finished)
 constexpr int kStepScratchBytes = 40 * 1024;      // shared memory of the row tasks (outside the operand ring)
 static_assert(8 * TC_EPI_STAGE_FLOATS * 4 <= kStepScratchBytes, "epilogue staging tiles live in the scratch area");
-constexpr int kStepSmemBytes = kStepStages * TC_STAGE_BYTES + kStepScratchBytes + 1024;
-constexpr int kStepTmemCols = 256;    // two 128-column accumulators
+// ring + row-task scratch + accumulator tile
+constexpr int kStepSmemBytes = kStepStages * TC_STAGE_BYTES + kStepScratchBytes + TC_ACC_BYTES + 1024;
 
 constexpr int kStepQueues = 8;
 
@@ -84,7 +87,7 @@ struct StepSlot {                // one scheduled task: descriptor + (GEMM) the 
 };
 
 // NOTE: polls use ld.relaxed, never ld.acquire: ptxas implements a gpu-scope acquire as load + CCTL.IVALL, i.e. every
-// poll invalidated the SM's whole L1 (187 k times per step, one every 0.4 us per SM: measured with ncu, profiles/).
+// poll invalidated the SM's whole L1, once per poll.
 // The acquire is one fence after the poll has succeeded.
 __device__ __forceinline__ void red_release(int* p, int v) {
   asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
@@ -106,16 +109,15 @@ __shared__ StepSlot g_slots[kStepSlots];
 
 // The tile epilogue of slot s, one out-of-line copy per class (own register allocation, see step_rows.cuh)
 template <int CLS>
-__device__ __noinline__ void step_epilogue_cls(const int s, const uint32_t tmem_base, const int acc, const int ew,
-                                               const uint32_t stage) {
+__device__ __noinline__ void step_epilogue_cls(const int s, const float* acc, const int ew, const uint32_t stage) {
   const StepSlot& sl = g_slots[s];
-  tc_epilogue_cls<8, CLS>(sl.ctx, sl.task.m0, sl.task.n0, sl.task.split, sl.n_iter, sl.task.mode, tmem_base, acc, ew, stage);
+  tc_epilogue_cls<8, CLS>(sl.ctx, sl.task.m0, sl.task.n0, sl.task.split, sl.n_iter, sl.task.mode, acc, ew, stage);
 }
 // TILE_REDUCE pass of slot s: the split-K partials of the tile, summed in split order, through the fused epilogue
 template <int CLS>
 __device__ __noinline__ void step_reduce_cls(const int s, const int ew, const uint32_t stage) {
   const StepSlot& sl = g_slots[s];
-  tc_epilogue_cls<8, CLS>(sl.ctx, sl.task.m0, sl.task.n0, 0, 0, TILE_REDUCE, 0u, 0, ew, stage);
+  tc_epilogue_cls<8, CLS>(sl.ctx, sl.task.m0, sl.task.n0, 0, 0, TILE_REDUCE, nullptr, ew, stage);
 }
 __device__ __forceinline__ void step_reduce(const int s, const int ew, const uint32_t stage) {
   if (epi_class(TILE_REDUCE, g_slots[s].ctx.g.flags) == EPI_CLS_PLAIN)
@@ -123,15 +125,14 @@ __device__ __forceinline__ void step_reduce(const int s, const int ew, const uin
   else
     step_reduce_cls<EPI_CLS_FORWARD>(s, ew, stage);      // split groups never carry auxiliary operands
 }
-__device__ __forceinline__ void step_epilogue(const int s, const uint32_t tmem_base, const int acc, const int ew,
-                                              const uint32_t stage) {
+__device__ __forceinline__ void step_epilogue(const int s, const float* acc, const int ew, const uint32_t stage) {
   const int cls = epi_class(g_slots[s].task.mode, g_slots[s].ctx.g.flags);
   if (cls == EPI_CLS_PLAIN)
-    step_epilogue_cls<EPI_CLS_PLAIN>(s, tmem_base, acc, ew, stage);
+    step_epilogue_cls<EPI_CLS_PLAIN>(s, acc, ew, stage);
   else if (cls == EPI_CLS_FORWARD)
-    step_epilogue_cls<EPI_CLS_FORWARD>(s, tmem_base, acc, ew, stage);
+    step_epilogue_cls<EPI_CLS_FORWARD>(s, acc, ew, stage);
   else
-    step_epilogue_cls<EPI_CLS_ALL>(s, tmem_base, acc, ew, stage);
+    step_epilogue_cls<EPI_CLS_ALL>(s, acc, ew, stage);
 }
 
 __device__ __forceinline__ int ld_relaxed(const int* p) {
@@ -228,34 +229,31 @@ __global__ void __launch_bounds__(kStepThreads, 1) ta3n_step_kernel(const __grid
   __shared__ int split_rank;            // TILE_SPLIT: how many splits of the tile had arrived before this one
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(step_smem_raw) + 1023) & ~uintptr_t(1023));
   float* scratch = reinterpret_cast<float*>(smem + kStepStages * TC_STAGE_BYTES);
+  float* acc_tile = reinterpret_cast<float*>(smem + kStepStages * TC_STAGE_BYTES + kStepScratchBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tid = threadIdx.x;
   int* const cursors = hd.counters + hd.n_counters;
   __shared__ int deferred[kStepDeferred];
 
   // ---- one-time setup ----
-  if (warp == 0 && lane == 0) {
-    tc_pipe_init<kStepStages>(&sh, 8);
+  if (warp == kStepProducerWarp && lane == 0) {
+    tc_pipe_init<kStepStages>(&sh);
     for (int s = 0; s < kStepSlots; ++s) {
       mbar_init(&slot_full[s], 1);
-      mbar_init(&slot_empty[s], 10);       // producer + MMA issuer + 8 epilogue warps
+      mbar_init(&slot_empty[s], 1 + TC_CONSUMER_WARPS);       // producer + 8 consumer warps
     }
     done_count = 0;
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&sh.tmem_slot, kStepTmemCols);
   for (int i = tid; i < (int)(sizeof(TailArgs) / sizeof(int)); i += kStepThreads)
     reinterpret_cast<int*>(&g_tail)[i] = reinterpret_cast<const int*>(hd.tail)[i];
   __syncthreads();
   if (tid == 0) g_tail.dbg = hd.trace ? hd.trace + (size_t)hd.n_tasks * 8 : nullptr;      // row-task phase marks
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = sh.tmem_slot;
   // (no griddepcontrol here: the kernel is launched with plain stream ordering behind the memset of its counters,
   //  and must not release its dependents before it has finished)
 
-  if (warp == 10) {
+  if (warp == kStepSchedulerWarp) {
     // =========================== scheduler: claim ready tasks, stage them ===========================
     int n_def = 0;
     for (uint32_t k = 0;; ++k) {
@@ -294,7 +292,7 @@ __global__ void __launch_bounds__(kStepThreads, 1) ta3n_step_kernel(const __grid
       __syncwarp();
       if (lane == 0) mbar_arrive(&slot_full[s]);
     }
-  } else if (warp == 0) {
+  } else if (warp == kStepProducerWarp) {
     // =========================== TMA producer ===========================
     if (lane == 0) {
       uint32_t slabs = 0;
@@ -313,32 +311,11 @@ __global__ void __launch_bounds__(kStepThreads, 1) ta3n_step_kernel(const __grid
         mbar_arrive(&slot_empty[s]);
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    if (lane == 0) {
-      uint32_t slabs = 0, tiles = 0;
-      for (uint32_t k = 0;; ++k) {
-        const int s = (int)(k % kStepSlots);
-        mbar_wait(&slot_full[s], (k / kStepSlots) & 1u);
-        const StepSlot& sl = slots[s];
-        const int type = sl.task.type;
-        if (type == TASK_STOP) break;
-        if (type == TASK_GEMM && sl.n_iter > 0) {
-          const int acc = (int)(tiles & 1u);
-          mbar_wait(&sh.tmem_empty_bar[acc], ((tiles >> 1) & 1u) ^ 1u);      // the epilogue has drained this buffer
-          tc_fence_after();
-          tc_mma<kStepStages>((sl.flags & 1) != 0, (sl.flags & 2) != 0, sl.n_iter, smem, &sh, tmem_base, acc, slabs);
-          slabs += (uint32_t)sl.n_iter;
-          ++tiles;
-        }
-        mbar_arrive(&slot_empty[s]);
-      }
-    }
   } else {
-    // =========================== epilogue / row warps (2..9) ===========================
-    const int ew = warp - 2;
-    const int rt = tid - 64;
-    uint32_t tiles = 0;
+    // =========================== consumer / epilogue / row warps (0..7) ===========================
+    const int ew = warp;
+    const int rt = tid;
+    uint32_t slabs = 0;
     for (uint32_t k = 0;; ++k) {
       const int s = (int)(k % kStepSlots);
       mbar_wait(&slot_full[s], (k / kStepSlots) & 1u);
@@ -349,18 +326,15 @@ __global__ void __launch_bounds__(kStepThreads, 1) ta3n_step_kernel(const __grid
       bool publish = true;                 // a split-K tile that was not the last to arrive has nothing to announce
       if (hd.trace && rt == 0) t_sched = global_ns();
       if (type == TASK_GEMM) {
-        const int acc = (int)(tiles & 1u);
-        if (sl.n_iter > 0) {
-          mbar_wait(&sh.tmem_full_bar[acc], (tiles >> 1) & 1u);
-          tc_fence_after();
+        if (sl.n_iter > 0) {            // (the previous task's readers of acc_tile are past the completion barrier)
+          float d[64];
+          tc_consume<kStepStages>((sl.flags & 1) != 0, (sl.flags & 2) != 0, sl.n_iter, smem, &sh, slabs, d);
+          slabs += (uint32_t)sl.n_iter;
+          tc_store_acc(acc_tile, d, tid);
+          row_sync();
         }
         if (hd.trace && rt == 0) t_acc = global_ns();
-        step_epilogue(s, tmem_base, acc, ew, smem_u32(scratch + ew * TC_EPI_STAGE_FLOATS));
-        if (sl.n_iter > 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&sh.tmem_empty_bar[acc]);      // this warp's TMEM reads are done
-          ++tiles;
-        }
+        step_epilogue(s, acc_tile, ew, smem_u32(scratch + ew * TC_EPI_STAGE_FLOATS));
         if (sl.task.mode == TILE_SPLIT) {      // raw partial written: am I the last split of this tile?
           row_sync();
           if (rt == 0) {
@@ -420,12 +394,6 @@ __global__ void __launch_bounds__(kStepThreads, 1) ta3n_step_kernel(const __grid
       __syncwarp();
       if (lane == 0) mbar_arrive(&slot_empty[s]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kStepTmemCols);
   }
 }
 

@@ -1,10 +1,10 @@
-// ta3n_api.cu -- extern "C" entry points of libta3n_sm100.so (see include/ta3n_b200.h).
+// ta3n_api.cu -- extern "C" entry points of libta3n_sm90.so (see include/ta3n_b200.h).
 // Every function only builds launch tables on the host and enqueues kernels on the caller's
 // stream: no allocation, no synchronisation, CUDA-graph capturable.
 #include "common.cuh"
 #include "seg_gemm.cuh"
 #include "rowops.cuh"
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include "optim.cuh"
 #include "step_plan.cuh"
 #include "allreduce.cuh"
@@ -976,7 +976,7 @@ int ta3n_step_run_phased(const ta3n_step_desc* desc, ta3n_stream_t stream) {
   StepProgram P;
   TA3N_TRY(build_step_program(desc, &P));
   cudaStream_t st = S(stream);
-  int sm_count = 148;
+  int sm_count = 132;
   TA3N_TRY(step_kernel_config(&sm_count));
   const int n_row = (P.M + kRowVideos - 1) / kRowVideos;
   auto rows = [&](const char* label, int kind) {
@@ -1066,7 +1066,7 @@ int ta3n_step_build(const ta3n_step_desc* desc, void* plan_dev, size_t plan_byte
   TA3N_REQUIRE((reinterpret_cast<uintptr_t>(plan_dev) & 255u) == 0, "plan buffer must be 256-byte aligned");
   StepProgram P;
   TA3N_TRY(build_step_program(desc, &P));
-  int sm_count = 148;
+  int sm_count = 132;
   TA3N_TRY(step_kernel_config(&sm_count));
   BuiltPlan B;
   float* partial = reinterpret_cast<float*>(static_cast<char*>(desc->workspace) + P.scratch_bytes);
@@ -1120,7 +1120,7 @@ int ta3n_step_run(const void* handle_host, ta3n_stream_t stream) {
   return after_launch();
 }
 
-// Host-only: the split-K factors the balanced planner (gemm_tcgen05.cuh: plan_splitk_balanced) would choose for a
+// Host-only: the split-K factors the balanced planner (gemm_wgmma.cuh: plan_splitk_balanced) would choose for a
 // precise forward launch of n_groups GEMMs C[M,N] += A[M,K] B[N,K]^T on `sms` SMs with `scratch_bytes` of forward
 // scratch; ksplit_out[n_groups] receives them, makespan_out[2] = {unsplit, chosen} makespan of the LPT model in K-slab
 // units.  No CUDA call: the planner's policy is testable on a machine without a GPU.
@@ -1155,7 +1155,7 @@ size_t ta3n_step_describe(const ta3n_step_desc* desc, char* buf, size_t buf_byte
   StepProgram P;
   if (build_step_program(desc, &P, /*dry=*/true) != TA3N_OK) return 0;
   BuiltPlan B;
-  if (build_task_graph(P, 148, nullptr, 0, &B) != TA3N_OK) return 0;
+  if (build_task_graph(P, 132, nullptr, 0, &B) != TA3N_OK) return 0;
   int n_type[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   long slabs = 0;
   int bad = 0;
@@ -1266,8 +1266,8 @@ int ta3n_allreduce_mean(float* const* peer_bufs_host, float* multicast_buf, uint
     const char* e = getenv("TA3N_AR_BLOCKS");
     return e ? atoi(e) : 0;
   }();
-  // measured at N=4 (cfg2 step, profiles/r2_allreduce_blocks.txt): 64 CTAs 0.411 ms/step, 32: 0.423, 128: 0.425 --
-  // fewer barrier participants, still enough loads in flight; two ranks use the peer path and want all 128
+  // from three ranks on 64 CTAs: fewer barrier participants, still enough loads in flight; two ranks use the peer
+  // path and want all 128 (chosen on an 8-GPU NVSwitch box of the previous generation; TA3N_AR_BLOCKS overrides)
   int blocks = env_blocks > 0 ? env_blocks : (world > 2 ? 64 : kArBlocks);
   blocks = std::max(1, std::min(blocks, kArBlocks));
   launch_kernel(allreduce_mean_kernel, blocks, kArThreads, 0, S(stream), P, multicast_buf,
@@ -1295,7 +1295,7 @@ int ta3n_sgd_nesterov_step_masked(float* params, const float* grads, float* mome
     TA3N_TRY(after_launch());
   }
   long long n4 = (n + 3) / 4;
-  int blocks = static_cast<int>(std::min<long long>((n4 + kOptThreads - 1) / kOptThreads, 148 * 8));
+  int blocks = static_cast<int>(std::min<long long>((n4 + kOptThreads - 1) / kOptThreads, 132 * 8));
   pre_launch("sgd_nesterov", S(stream));
   launch_kernel(sgd_nesterov_kernel, blocks, kOptThreads, 0, S(stream), params, grads, momentum_buf, n, lr_dev,
                 momentum, weight_decay, max_norm, static_cast<const float*>(partial), kSqnormBlocks, stats, active);

@@ -3,7 +3,7 @@
 Same constructor signature (models.py:59-67), same ``forward(input_source, input_target, beta,
 mu, is_train, reverse)`` -> 10-tuple contract (models.py:545, 722), same parameter names and
 shapes (so reference checkpoints load), same initialisation order under a given seed.
-All arithmetic runs in libta3n_sm100.so; options outside the hot path raise NotImplementedError.
+All arithmetic runs in libta3n_sm90.so; options outside the hot path raise NotImplementedError.
 """
 from __future__ import annotations
 

@@ -96,10 +96,10 @@ def flatten_parameters(model) -> torch.Tensor:
 
 class TrainStep:
     """Options ``overlap_wgrad`` / ``parallel_branches`` put independent parts of the backward on forked streams
-    inside the captured graph.  Measured on B200: forked sub-wave tcgen05 GEMM nodes of one graph do not overlap under
-    plain tf32 (tools/concurrency_probe.py: 49.9 us forked vs 50.4 us sequential for two 80-tile launches), so
+    inside the captured graph.  Forked sub-wave tensor-core GEMM nodes of one graph were found not to overlap under
+    plain tf32 (tools/concurrency_probe.py measures it), so
     ``parallel_branches`` is off by default; ``overlap_wgrad`` defaults to on only under the tf32x3 engine, where the
-    small precise weight-gradient launch hides behind the data-gradient chain (tools/legacy_options.py: -12 us)."""
+    small precise weight-gradient launch hides behind the data-gradient chain (tools/legacy_options.py)."""
 
     def __init__(self, model, batch_source: int, batch_target: int, beta: Sequence[float], gamma: float = 0.003,
                  place_adv: Sequence[str] = ("Y", "Y", "Y"), add_loss_DA: str = "attentive_entropy",
@@ -272,12 +272,11 @@ class TrainStep:
         self.branch_stream = torch.cuda.Stream(device=dev) if parallel_branches else None
         self.overlap_wgrad = bool(overlap_wgrad)
         self.side_stream = torch.cuda.Stream(device=dev) if self.overlap_wgrad else None
-        # measured at N=2 (profiles/r2_bench_n2_early_allreduce.txt): 0.448 ms/step with the early bucket reduced on a
-        # forked stream against 0.432 with one all-reduce behind the step -- the collective is latency / rank-skew bound
-        # (a second kernel pays the fixed ~25 us again and competes for SMs), so the split is opt-in
+        # reducing the early bucket on a forked stream was slower than one all-reduce behind the step -- the collective is
+        # latency / rank-skew bound (a second kernel pays the fixed cost again and competes for SMs), so the split is opt-in
         self.early_ar = os.environ.get("TA3N_EARLY_ALLREDUCE", "0") == "1"
         self.ar_stream = torch.cuda.Stream(device=dev) if (self.overlap_wgrad and self.ar is not None) else None
-        self.launches_per_step = 0               # kernels of libta3n_sm100.so per step (counted at capture)
+        self.launches_per_step = 0               # kernels of libta3n_sm90.so per step (counted at capture)
         self.use_graph = bool(use_graph)
         self.graphs = [None] * self.n_slots      # per input slot: (graph_a, graph_b or None)
         self.step_descs = [None] * self.n_slots  # fused / phased: ta3n_step_desc per input slot (+ keep-alives)
@@ -320,8 +319,8 @@ class TrainStep:
             torch.cuda.synchronize()
             dist.barrier(group=self.group)              # every rank's flags are zero before anybody signals
             mc = int(getattr(hdl, "multicast_ptr", 0) or 0)
-            # two ranks: plain peer loads / stores are faster than the switch reduction (50 vs 61 us back to back,
-            # 13.9 MB; at eight ranks 80 vs 67: tools/allreduce_probe.py, profiles/r2_allreduce_probe_n*.txt)
+            # two ranks: plain peer loads / stores are faster than the switch reduction; from three ranks on the multicast
+            # reduction wins (tools/allreduce_probe.py)
             if os.environ.get("TA3N_ALLREDUCE_NO_MULTICAST") == "1" or (self.world <= 2 and
                                                                          os.environ.get("TA3N_ALLREDUCE_MULTICAST") != "1"):
                 mc = 0

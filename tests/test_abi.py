@@ -18,7 +18,7 @@ def declared_functions():
 @pytest.fixture(scope="module")
 def lib():
     from ta3n_b200 import build
-    build.build()                       # nvcc cross-compiles sm_100a without a GPU
+    build.build()                       # nvcc cross-compiles sm_90a without a GPU
     from ta3n_b200 import _lib
     return _lib.load()
 

@@ -8,7 +8,6 @@ import torch
 
 from oracle import dataset_oracle as dorc
 from oracle import gen_golden_dataset as gg
-from oracle import ref_shims
 from ta3n_b200 import dataset as D
 
 GOLDEN = np.load(gg.GOLDEN_PATH)
@@ -34,38 +33,24 @@ def test_index_rules_match_reference_golden(rule):
                 assert got.shape == want.shape and np.array_equal(got.astype(np.int64), want), (rule, key, fn.__module__)
 
 
-def _make_tree(root, n_videos=7, feat_dim=16, seed=3):
-    """A miniature dataset in the reference's on-disk format: <root>/vK/img_00001.t7 ... one tensor per frame."""
-    g = torch.Generator().manual_seed(seed)
-    lines = []
-    for v in range(n_videos):
-        nf = int(torch.randint(2, 14, (1,), generator=g))
-        d = os.path.join(root, f"v{v}")
-        os.makedirs(d)
-        for f in range(1, nf + 1):
-            torch.save(torch.randn(feat_dim, generator=g), os.path.join(d, "img_{:05d}.t7".format(f)))
-        lines.append(f"{d} {nf} {v % 3}")
-    lst = os.path.join(root, "list.txt")
-    with open(lst, "w") as fh:
-        fh.write("\n".join(lines) + "\n")
-    return lst
+_make_tree = dorc.make_feature_tree
 
 
-@pytest.mark.skipif(not ref_shims.available(), reason="/root/reference not present")
 @pytest.mark.parametrize("mode", ["test", "val", "random"])
 def test_tsn_dataset_equals_live_reference(tmp_path, mode):
+    """TSNDataSet against the reference's TSNDataSet on the same miniature tree: its items are stored in
+    tests/golden/reference_pins.npz (oracle/gen_golden_pins.py)."""
+    pins = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_pins.npz"))
     lst = _make_tree(str(tmp_path))
-    ref_mod = ref_shims.load_dataset()
     kw = dict(num_dataload=10, num_segments=5, new_length=1, modality="RGB",
               random_shift=(mode == "random"), test_mode=(mode == "test"))
-    ref, mine = ref_mod.TSNDataSet("", lst, **kw), D.TSNDataSet("", lst, **kw)
-    assert len(ref) == len(mine) == 10                         # list tiled to num_dataload (dataset.py:70-75)
-    for i in range(len(ref)):
-        np.random.seed(100 + i)
-        xr, yr = ref[i]
+    mine = D.TSNDataSet("", lst, **kw)
+    assert len(mine) == 10                                     # list tiled to num_dataload (dataset.py:70-75)
+    for i in range(len(mine)):
         np.random.seed(100 + i)
         xm, ym = mine[i]
-        assert yr == ym and torch.equal(xr, xm), (mode, i)
+        xr, yr = pins[f"dataset/{mode}/{i}/x"], int(pins[f"dataset/{mode}/{i}/y"])
+        assert yr == ym and np.array_equal(xm.numpy(), xr), (mode, i)
 
 
 def test_packed_shard_serves_the_same_items(tmp_path):

@@ -17,7 +17,7 @@ from tests.golden_util import (TOL_PATH, abs_err, assert_close, check_grads_agai
 
 pytestmark = pytest.mark.gpu
 
-# Engines: "fp32" = exact SIMT tiles; "tf32x3" = the PRODUCT engine (tcgen05; forward layers at fp32 grade, backward
+# Engines: "fp32" = exact SIMT tiles; "tf32x3" = the PRODUCT engine (wgmma; forward layers at fp32 grade, backward
 # GEMMs plain tf32); "tf32" = plain tf32 everywhere (fastest; its forward error flips ~1e-4 of the ReLU units, which
 # costs 1-2 % of gradient accuracy -- kept as an option, held to a documented looser bound).
 ENGINES = ["fp32", "tf32x3", "tf32"]
@@ -272,7 +272,7 @@ def test_avgpool_variant_matches_oracle(T, fc_dim, bs, bt, use_attn, ens, engine
 @pytest.mark.parametrize("T,attn_frame,bs,bt", [(5, "none", 48, 40), (6, "TransAttn", 12, 20)])
 def test_tf32_gradients_match_oracle_on_realised_activation_pattern(T, attn_frame, bs, bt):
     """tf32 engine: with the ReLU on/off pattern of the CUDA forward pinned in the fp64 oracle, the loss
-    agrees to 1e-3 and every parameter gradient to 3e-3 (measured <= 5e-4 at cfg2, profiles/r1_parity_report.txt) -- the extra 1-2.5 % seen without pinning comes only from the
+    agrees to 1e-3 and every parameter gradient to 3e-3 -- the extra 1-2.5 % seen without pinning comes only from the
     handful of units whose pre-activation is within tf32 rounding error of zero."""
     import ta3n_b200
     from ta3n_b200.train import TrainStep

@@ -1,4 +1,4 @@
-"""Host logic of the tf32x3 engine's balanced split-K planner (csrc/gemm_tcgen05.cuh: plan_splitk_balanced), through the
+"""Host logic of the tf32x3 engine's balanced split-K planner (csrc/gemm_wgmma.cuh: plan_splitk_balanced), through the
 host-only C-ABI entry ta3n_plan_forward_splits.  No GPU: the planner only does arithmetic on shapes."""
 import itertools
 
@@ -6,7 +6,7 @@ import pytest
 
 from ta3n_b200 import _lib
 
-BK = 32                     # K slab of the tcgen05 kernels (TC_BK)
+BK = 32                     # K slab of the tensor-core kernels (TC_BK)
 SHARED_CFG2 = [(2560, 512, 2048)]           # shared layer at cfg2: (Bs+Bt)*T = 2560 rows, 80 tiles of 64 slabs
 FWD_BATCH_LIKE = [(2560, 256, 512)] + [(640, 256, 512 * r) for r in (2, 3, 4, 5)]     # short tiles next to long ones
 
@@ -32,8 +32,8 @@ def test_split_factors_are_admissible(shapes):
 
 
 def test_underfilled_grid_gets_split():
-    # 80 tiles on 148 SMs: unsplit, 68 SMs idle and the launch lasts one full tile (64 slabs + overhead)
-    ks, before, after = _lib.plan_forward_splits(SHARED_CFG2, sms=148)
+    # 80 tiles on 132 SMs: unsplit, 52 SMs idle and the launch lasts one full tile (64 slabs + overhead)
+    ks, before, after = _lib.plan_forward_splits(SHARED_CFG2, sms=132)
     assert before == pytest.approx(68.0)
     assert ks[0] >= 2 and after < 0.8 * before
 

@@ -1,4 +1,4 @@
-"""Do two independent sub-wave tcgen05 GEMM launches overlap when captured on forked streams?"""
+"""Do two independent sub-wave tensor-core GEMM launches overlap when captured on forked streams?"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, ta3n_b200

@@ -1,4 +1,4 @@
-"""Time the tcgen05 GEMM engine in isolation: N back-to-back launches captured in one CUDA graph."""
+"""Time the tensor-core GEMM engine in isolation: N back-to-back launches captured in one CUDA graph."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -18,4 +18,4 @@ for (M, N, K) in [(128, 128, 32), (512, 256, 256)]:
     g.replay(); torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(); g.replay(); g.replay(); e1.record(); torch.cuda.synchronize()
-    print(f"dbg={os.environ.get('TA3N_TC_DEBUG','0'):>3s} M={M} N={N} K={K}: {e0.elapsed_time(e1)*1e3/(2*REP):7.2f} us/launch")
+    print(f"M={M} N={N} K={K}: {e0.elapsed_time(e1)*1e3/(2*REP):7.2f} us/launch")
