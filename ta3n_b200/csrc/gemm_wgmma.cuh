@@ -16,6 +16,12 @@
 //                                 warps transpose the stage in place into the K-major layout above before the MMAs.
 // After the K loop the accumulators pass through a row-major shared-memory tile (TC_ACC_LD floats per row), from
 // which every epilogue warp reads whole 32-column row pieces.
+//
+// The precise forward kernel (seg_gemm_tc_x3_kernel, "tf32x3") adds a producer warpgroup: 384 threads, warp 8 for
+// TMA and warps 9..11 that write the tf32 lo tile of each landed B tile (transposing MN-major B on the way).  Its
+// consumers take A from registers: each thread loads its own fragment words from the raw stage and splits them
+// there, so the MMA warps do nothing but load, split and issue in the K loop.  setmaxnreg gives the producer
+// warpgroup 40 registers per thread and the consumers 232.
 #pragma once
 
 #include <cuda.h>
@@ -148,6 +154,32 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint6
       : "l"(adesc), "l"(bdesc), "r"(1)
       : "memory");
 }
+// The same product with A from registers: fragment of thread (warp w of the warpgroup, lane l) a[j] = A(row
+// 16w + l/4 + 8(j&1), column l%4 + 4(j>>1)).  The registers must not be written until a wgmma.wait_group has
+// retired the MMA.
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[64], const uint32_t a0, const uint32_t a1, const uint32_t a2,
+                                              const uint32_t a3, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(1)
+      : "memory");
+}
+// pins a register value at this point of the instruction stream (before a wgmma.fence that must cover its write)
+__device__ __forceinline__ void reg_fence(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+__device__ __forceinline__ float lds1(uint32_t saddr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(saddr) : "memory");
+  return v;
+}
+// warpgroup register budget (every thread of the warpgroup executes it)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ---- operand tiles as the tensor core reads them ---------------------------------------------------------
 // byte offset of the 16 B chunk holding k = 4kq .. 4kq+3 of row m in a K-major SW128 tile
@@ -159,56 +191,38 @@ __device__ __forceinline__ uint32_t mnmaj_chunk(int k, int mq) {
 __device__ __forceinline__ float tf32_hi(float a) { return __uint_as_float(__float_as_uint(a) & 0xFFFFE000u); }
 __device__ __forceinline__ float f4_at(const float4& v, int i) { return i == 0 ? v.x : i == 1 ? v.y : i == 2 ? v.z : v.w; }
 
-// One operand tile of a landed stage (consumer thread t of 256 owns four 16 B chunks).  MN-major: a 4 x 4 block
-// (m = 4mq.., k = 4kq..), read here, written transposed by tc_prep_store; the lane -> block map keeps the 16 B
-// stores conflict-free and the loads at most 2-way.
+// One 4 x 4 block (m = 4mq.., k = 4kq..) of an MN-major operand tile, block t of 256: read by tc_prep_load, written
+// K-major (transposed) by tc_prep_store; the block map keeps the 16 B stores of 32 consecutive blocks conflict-free
+// and the loads at most 2-way.
 __device__ __forceinline__ void tc_prep_blk(const int t, int* mq, int* kq) {
   *mq = (t & 1) | (((t >> 3) & 15) << 1);
   *kq = ((t >> 1) & 3) | (((t >> 7) & 1) << 2);
 }
-__device__ __forceinline__ void tc_prep_load(const uint32_t base, const bool kmaj, const int t, float4 (&r)[4]) {
+__device__ __forceinline__ void tc_prep_load(const uint32_t base, const int t, float4 (&r)[4]) {
   int mq, kq;
   tc_prep_blk(t, &mq, &kq);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) r[i] = lds4(base + (kmaj ? (uint32_t)(t + 256 * i) * 16u : mnmaj_chunk(4 * kq + i, mq)));
+  for (int i = 0; i < 4; ++i) r[i] = lds4(base + mnmaj_chunk(4 * kq + i, mq));
 }
-// split: write hi (the bits the tensor core reads) in place and lo = a - hi (exact) `lo_off` bytes further
-__device__ __forceinline__ void tc_prep_put(const uint32_t addr, const float4 v, const bool split, const uint32_t lo_off) {
-  if (!split) {
-    sts4(addr, v);
-    return;
-  }
-  const float4 h = make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w));
-  sts4(addr, h);
-  sts4(addr + lo_off, make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w));
-}
-__device__ __forceinline__ void tc_prep_store(const uint32_t base, const bool kmaj, const int t, const float4 (&r)[4],
-                                              const bool split, const uint32_t lo_off) {
+__device__ __forceinline__ void tc_prep_store(const uint32_t base, const int t, const float4 (&r)[4]) {
   int mq, kq;
   tc_prep_blk(t, &mq, &kq);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    if (kmaj) {
-      tc_prep_put(base + (uint32_t)(t + 256 * i) * 16u, r[i], split, lo_off);
-    } else {
-      const float4 w = make_float4(f4_at(r[0], i), f4_at(r[1], i), f4_at(r[2], i), f4_at(r[3], i));
-      tc_prep_put(base + kmaj_chunk(4 * mq + i, kq), w, split, lo_off);
-    }
-  }
+  for (int i = 0; i < 4; ++i)
+    sts4(base + kmaj_chunk(4 * mq + i, kq), make_float4(f4_at(r[0], i), f4_at(r[1], i), f4_at(r[2], i), f4_at(r[3], i)));
 }
-// Make a landed stage readable by wgmma: MN-major operands transposed in place; `split` (precise kernel): every operand
-// as hi / lo tiles.  Called by all 256 consumer threads; ends with the stage visible to the tensor core.
+// Make a landed stage readable by wgmma: MN-major operands transposed in place.  Called by all 256 consumer threads;
+// ends with the stage visible to the tensor core.
 __device__ __forceinline__ void tc_prep_stage(const uint32_t a_base, const uint32_t b_base, const bool a_kmaj,
-                                              const bool b_kmaj, const bool split, const uint32_t lo_off) {
-  const bool pa = !a_kmaj || split, pb = !b_kmaj || split;
-  if (!pa && !pb) return;
+                                              const bool b_kmaj) {
+  if (a_kmaj && b_kmaj) return;
   const int t = threadIdx.x;
   float4 ra[4], rb[4];
-  if (pa) tc_prep_load(a_base, a_kmaj, t, ra);
-  if (pb) tc_prep_load(b_base, b_kmaj, t, rb);
-  if (!a_kmaj || !b_kmaj) consumer_sync();          // every read of the stage before the in-place transposed writes
-  if (pa) tc_prep_store(a_base, a_kmaj, t, ra, split, lo_off);
-  if (pb) tc_prep_store(b_base, b_kmaj, t, rb, split, lo_off);
+  if (!a_kmaj) tc_prep_load(a_base, t, ra);
+  if (!b_kmaj) tc_prep_load(b_base, t, rb);
+  consumer_sync();                                  // every read of the stage before the in-place transposed writes
+  if (!a_kmaj) tc_prep_store(a_base, t, ra);
+  if (!b_kmaj) tc_prep_store(b_base, t, rb);
   fence_proxy_async();                              // generic-proxy writes -> the tensor core's reads
   consumer_sync();
 }
@@ -339,7 +353,7 @@ __device__ __forceinline__ void tc_consume(const bool a_kmaj, const bool b_kmaj,
     mbar_wait(&sh->full_bar[stage], (gl / STAGES) & 1u);
     const uint32_t a_base = smem_u32(smem + stage * TC_STAGE_BYTES);
     const uint32_t b_base = a_base + TC_A_BYTES;
-    tc_prep_stage(a_base, b_base, a_kmaj, b_kmaj, false, 0u);
+    tc_prep_stage(a_base, b_base, a_kmaj, b_kmaj);
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < TC_BK / 8; ++ks) wgmma_tf32(d, wgmma_desc(a_base + wg * 64 * 128, ks), wgmma_desc(b_base, ks));
@@ -739,20 +753,126 @@ seg_gemm_tc_kernel(const __grid_constant__ GemmTable tab, const __grid_constant_
 //     full K = 2048 the tensor core's own accumulation limits the result to ~5e-6 whatever the operands; chunked, the
 //     error of an fp32 FFMA loop;
 //   * the tensor maps deliver the RAW fp32 words (no TMA rounding), so that hi + lo = a exactly.
-// The consumer warps write the hi / lo tiles of each landed stage (shared memory -> shared memory, transposing
-// MN-major operands on the way), run the three products, and fold every finished chunk into 64 running sums.
-constexpr int X3_STAGES = 3;
-constexpr int X3_STAGE_BYTES = 2 * TC_STAGE_BYTES;            // [A | B | A_lo | B_lo]
+// Roles (384 threads): warp 8 lane 0 issues the TMA loads of the raw words; warps 9..11 write the lo tile of each
+// landed B tile beside it (the raw tile serves as hi), transposing MN-major B on the way, and mark the stage ready;
+// the two consumer warpgroups load their A fragments from the raw stage into registers, split them there, and issue
+// the three products with B from shared memory.  The consumer warps do nothing else in the K loop; they fold every
+// finished chunk into 64 running sums.  setmaxnreg moves registers from the producer warpgroup to the consumers,
+// which hold 64 accumulators, 64 sums and two slabs of A fragments (hi and lo).
+constexpr int X3_THREADS = 384;                               // warps 0..7 consumers, 8 TMA, 9..11 B split
+constexpr int X3_SPLIT_WARPS = 3;
+constexpr int X3_SPLIT_THREADS = 32 * X3_SPLIT_WARPS;
+// one CTA per SM: 65536 / 384 threads, rounded down to the allocation unit of 8, is 168 registers per thread at launch
+constexpr int X3_PRODUCER_REGS = 40, X3_CONSUMER_REGS = 232;
+static_assert(128 * X3_PRODUCER_REGS + 256 * X3_CONSUMER_REGS <= X3_THREADS * 168,
+              "setmaxnreg budget exceeds the registers of one CTA");
+constexpr int X3_STAGES = 4;
+constexpr int X3_STAGE_BYTES = TC_STAGE_BYTES + TC_B_BYTES;   // [A raw | B raw (= B hi) | B lo]
 constexpr int X3_CHUNK = 8;                                   // slabs (256 K columns) per tensor-core accumulation
+static_assert(X3_CHUNK % 2 == 0, "the A fragment register sets alternate by slab within a chunk");
 constexpr int x3_smem_bytes() { return X3_STAGES * X3_STAGE_BYTES + 1024; }
 static_assert(TC_ACC_BYTES <= X3_STAGES * X3_STAGE_BYTES, "the precise kernel reuses its operand ring");
 
+// the 96 split threads only
+__device__ __forceinline__ void x3_split_sync() { asm volatile("bar.sync 2, 96;" ::: "memory"); }
+
+// Split warps (thread t of 96): lo = b - hi of the B tile of a landed stage, K-major SW128 at b_lo.  The hi tile is
+// the raw K-major tile at b_raw itself: the tensor core reads an fp32 word as tf32 by ignoring its low 13 mantissa
+// bits, which is hi exactly, so only lo is written.  MN-major B is first transposed into the lo tile and then written
+// back K-major at b_raw on the way.
+template <bool B_KMAJ>
+__device__ __forceinline__ void x3_split_b(const uint32_t b_raw, const uint32_t b_lo, const int t) {
+  uint32_t src = b_raw;
+  if (!B_KMAJ) {
+#pragma unroll 1
+    for (int blk = t; blk < 256; blk += X3_SPLIT_THREADS) {
+      float4 r[4];
+      tc_prep_load(b_raw, blk, r);
+      tc_prep_store(b_lo, blk, r);
+    }
+    x3_split_sync();                  // every read of the raw tile before the K-major writes over it
+    src = b_lo;
+  }
+#pragma unroll 2
+  for (int c = t; c < TC_B_BYTES / 16; c += X3_SPLIT_THREADS) {
+    const float4 v = lds4(src + 16u * c);
+    if (!B_KMAJ) sts4(b_raw + 16u * c, v);
+    sts4(b_lo + 16u * c, make_float4(v.x - tf32_hi(v.x), v.y - tf32_hi(v.y), v.z - tf32_hi(v.z), v.w - tf32_hi(v.w)));
+  }
+}
+
+// Per-thread part of the A fragment addresses of rows m = r0 (and r0 + 8, MN-major), column k = tq: the word offset
+// in the raw tile, whose bits 4..6 are the SW128 chunk index.  Stage bases are 1024-B aligned, so x3_load_a reaches
+// every other column by an XOR on those bits plus a constant, with no per-column offsets kept in registers.
+template <bool A_KMAJ>
+__device__ __forceinline__ uint32_t x3_a_thread_off(const int m, const int tq) {
+  return A_KMAJ ? kmaj_chunk(m, 0) + 4u * tq : mnmaj_chunk(tq, m >> 2) + 4u * (m & 3);
+}
+
+// Consumer thread: the A fragments of one slab (4 k-steps x 4 words, see wgmma_tf32_rs) from the raw stage, split
+// into hi and lo.  K-major loads are conflict-free (the SW128 chunk index differs per row), MN-major ones 2-way.
+//   K-major  (m, k = 8 ks + 4 half + tq): (a_raw + off0) ^ ((2 ks + half) << 4), + 1024 for row r0 + 8 (same m & 7)
+//   MN-major (m, k = 8 ks + 4 half + tq): (a_raw + off_m) ^ (half << 6), + 128 (4 half + 8 ks) k-rows
+template <bool A_KMAJ>
+__device__ __forceinline__ void x3_load_a(const uint32_t a_raw, const uint32_t off0, const uint32_t off1,
+                                          uint32_t (&hi)[16], uint32_t (&lo)[16]) {
+  const uint32_t p0 = a_raw + off0, p1 = a_raw + off1;
+#pragma unroll
+  for (int ks = 0; ks < TC_BK / 8; ++ks)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint32_t row = j & 1, half = j >> 1;
+      const uint32_t addr = A_KMAJ ? (p0 ^ ((2u * ks + half) << 4)) + 1024u * row
+                                   : ((row ? p1 : p0) ^ (half << 6)) + 512u * half + 1024u * ks;
+      const float a = lds1(addr);
+      const float h = tf32_hi(a);
+      hi[4 * ks + j] = __float_as_uint(h);
+      lo[4 * ks + j] = __float_as_uint(a - h);
+    }
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    reg_fence(hi[j]);
+    reg_fence(lo[j]);
+  }
+}
+
+// Consumer warpgroups: slab `it` of the tile.  The fragments (hi, lo) must not belong to the group still in flight:
+// the caller alternates two register sets.  Leaves this slab's group in flight and releases the previous stage.
+template <bool A_KMAJ>
+__device__ __forceinline__ void x3_consume_slab(const int it, uint8_t* smem, TcShared* sh, uint64_t* ready_bar,
+                                                const uint32_t off0, const uint32_t off1, uint32_t (&hi)[16],
+                                                uint32_t (&lo)[16], float (&d)[64], int& prev) {
+  const int stage = it % X3_STAGES;
+  const uint32_t parity = (uint32_t)(it / X3_STAGES) & 1u;
+  mbar_wait(&sh->full_bar[stage], parity);          // raw A landed (read below with ordinary loads)
+  mbar_wait(&ready_bar[stage], parity);             // B lo (and transposed MN-major B) written
+  const uint32_t a_raw = smem_u32(smem + stage * X3_STAGE_BYTES);
+  const uint32_t b_hi = a_raw + TC_A_BYTES, b_lo = b_hi + TC_B_BYTES;
+  x3_load_a<A_KMAJ>(a_raw, off0, off1, hi, lo);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < TC_BK / 8; ++ks) {          // small terms first
+    const int f = 4 * ks;
+    wgmma_tf32_rs(d, lo[f], lo[f + 1], lo[f + 2], lo[f + 3], wgmma_desc(b_hi, ks));
+    wgmma_tf32_rs(d, hi[f], hi[f + 1], hi[f + 2], hi[f + 3], wgmma_desc(b_lo, ks));
+    wgmma_tf32_rs(d, hi[f], hi[f + 1], hi[f + 2], hi[f + 3], wgmma_desc(b_hi, ks));
+  }
+  wgmma_commit();
+  wgmma_wait<1>();                                  // the previous slab's MMAs are done: release its stage
+  if (prev >= 0) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&sh->empty_bar[prev]);
+  }
+  prev = stage;
+}
+
 template <bool A_KMAJ, bool B_KMAJ>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+__global__ void __launch_bounds__(X3_THREADS, 1)
 seg_gemm_tc_x3_kernel(const __grid_constant__ GemmTable tab, const __grid_constant__ TcMaps maps,
                       const __grid_constant__ TcSegMaps segmaps) {
   extern __shared__ uint8_t tc_smem_raw[];
   __shared__ __align__(8) TcShared sh;
+  __shared__ __align__(8) uint64_t ready_bar[X3_STAGES];     // B split done (one arrival per split warp)
   __shared__ TileCtx ctx;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -763,46 +883,47 @@ seg_gemm_tc_x3_kernel(const __grid_constant__ GemmTable tab, const __grid_consta
   tc_decode(ctx, tile, &split, &m0, &n0);
   tc_chunk_range(ctx, split, &c_begin, &n_iter);
 
-  if (warp == TC_CONSUMER_WARPS && lane == 0) tc_pipe_init<X3_STAGES>(&sh);
+  if (warp == TC_CONSUMER_WARPS && lane == 0) {
+    for (int s = 0; s < X3_STAGES; ++s) mbar_init(&ready_bar[s], X3_SPLIT_WARPS);
+    tc_pipe_init<X3_STAGES>(&sh);
+  }
   __syncthreads();
   pdl_wait();
 
-  const int mode = ctx.g.ksplit > 1 ? TILE_PARTIAL : TILE_FINAL;
-  if (warp == TC_CONSUMER_WARPS) {
-    if (lane == 0 && n_iter > 0)
-      tc_produce<X3_STAGES, X3_STAGE_BYTES>(ctx, maps.m, A_KMAJ, B_KMAJ, tab.pad_, m0, n0, c_begin, n_iter, smem, &sh, 0u);
+  if (warp >= TC_CONSUMER_WARPS) {
+    setmaxnreg_dec<X3_PRODUCER_REGS>();
+    if (warp == TC_CONSUMER_WARPS) {
+      if (lane == 0 && n_iter > 0)
+        tc_produce<X3_STAGES, X3_STAGE_BYTES>(ctx, maps.m, A_KMAJ, B_KMAJ, tab.pad_, m0, n0, c_begin, n_iter, smem, &sh,
+                                              0u);
+    } else {
+      const int t = threadIdx.x - 32 * (TC_CONSUMER_WARPS + 1);
+      for (int it = 0; it < n_iter; ++it) {
+        const int stage = it % X3_STAGES;
+        mbar_wait(&sh.full_bar[stage], (uint32_t)(it / X3_STAGES) & 1u);
+        const uint32_t b_raw = smem_u32(smem + stage * X3_STAGE_BYTES) + TC_A_BYTES;
+        x3_split_b<B_KMAJ>(b_raw, b_raw + TC_B_BYTES, t);
+        fence_proxy_async();            // generic-proxy writes -> the tensor core's reads
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&ready_bar[stage]);
+      }
+    }
   } else {
-    const int wg = threadIdx.x >> 7;
+    setmaxnreg_inc<X3_CONSUMER_REGS>();
+    const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);      // fragment rows r0, r0 + 8
+    const uint32_t off0 = x3_a_thread_off<A_KMAJ>(r0, lane & 3), off1 = x3_a_thread_off<A_KMAJ>(r0 + 8, lane & 3);
     float d[64], sum[64];
 #pragma unroll
     for (int j = 0; j < 64; ++j) d[j] = sum[j] = 0.f;
-    // One group of MMAs stays in flight while the next stage is split; at the end of a chunk every MMA must have
-    // finished before the fold reads the accumulator.
+    uint32_t hi[2][16], lo[2][16];      // A fragments of the even / odd slabs of a chunk
+    // One group of MMAs stays in flight while the next slab's fragments are loaded; at the end of a chunk every MMA
+    // must have finished before the fold reads the accumulator.
     int prev = -1;                      // stage whose MMAs may still be in flight
     for (int c0 = 0; c0 < n_iter; c0 += X3_CHUNK) {
       const int c1 = min(n_iter, c0 + X3_CHUNK);
-      for (int it = c0; it < c1; ++it) {
-        const int stage = it % X3_STAGES;
-        mbar_wait(&sh.full_bar[stage], (uint32_t)(it / X3_STAGES) & 1u);
-        const uint32_t a_hi = smem_u32(smem + stage * X3_STAGE_BYTES);
-        const uint32_t b_hi = a_hi + TC_A_BYTES;
-        const uint32_t a_lo = a_hi + TC_STAGE_BYTES, b_lo = b_hi + TC_STAGE_BYTES;
-        tc_prep_stage(a_hi, b_hi, A_KMAJ, B_KMAJ, true, TC_STAGE_BYTES);
-        const uint32_t arow = (uint32_t)wg * 64u * 128u;
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < TC_BK / 8; ++ks) {                      // small terms first
-          wgmma_tf32(d, wgmma_desc(a_lo + arow, ks), wgmma_desc(b_hi, ks));
-          wgmma_tf32(d, wgmma_desc(a_hi + arow, ks), wgmma_desc(b_lo, ks));
-          wgmma_tf32(d, wgmma_desc(a_hi + arow, ks), wgmma_desc(b_hi, ks));
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                // the previous stage's MMAs are done: release it
-        if (prev >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&sh.empty_bar[prev]);
-        }
-        prev = stage;
+      for (int it = c0; it < c1; it += 2) {
+        x3_consume_slab<A_KMAJ>(it, smem, &sh, ready_bar, off0, off1, hi[0], lo[0], d, prev);
+        if (it + 1 < c1) x3_consume_slab<A_KMAJ>(it + 1, smem, &sh, ready_bar, off0, off1, hi[1], lo[1], d, prev);
       }
       wgmma_wait<0>();                  // chunk complete: fold it into the fp32 sums
       __syncwarp();
@@ -818,7 +939,12 @@ seg_gemm_tc_x3_kernel(const __grid_constant__ GemmTable tab, const __grid_consta
     float* acc = reinterpret_cast<float*>(smem);
     tc_store_acc(acc, sum, threadIdx.x);
     consumer_sync();
-    tc_epilogue<TC_CONSUMER_WARPS>(ctx, m0, n0, split, n_iter, mode, acc, warp);
+    // the tile coordinates again from the staged context: kept live across the K loop they cost registers there
+    int e_split, e_m0, e_n0, e_begin, e_iter;
+    tc_decode(ctx, tile, &e_split, &e_m0, &e_n0);
+    tc_chunk_range(ctx, e_split, &e_begin, &e_iter);
+    tc_epilogue<TC_CONSUMER_WARPS>(ctx, e_m0, e_n0, e_split, e_iter, ctx.g.ksplit > 1 ? TILE_PARTIAL : TILE_FINAL, acc,
+                                   warp);
   }
 }
 
@@ -977,7 +1103,7 @@ inline int tc_launch_x3(const GemmTable& tab, const TcMaps& maps, const TcSegMap
     }
   }
   pre_launch(label, stream);
-  launch_kernel(seg_gemm_tc_x3_kernel<A_KMAJ, B_KMAJ>, tab.total_tiles, TC_THREADS, x3_smem_bytes(), stream, tab, maps, sm);
+  launch_kernel(seg_gemm_tc_x3_kernel<A_KMAJ, B_KMAJ>, tab.total_tiles, X3_THREADS, x3_smem_bytes(), stream, tab, maps, sm);
   return after_launch();
 }
 
