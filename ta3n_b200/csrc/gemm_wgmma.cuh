@@ -21,7 +21,9 @@
 // TMA and warps 9..11 that write the tf32 lo tile of each landed B tile (transposing MN-major B on the way).  Its
 // consumers take A from registers: each thread loads its own fragment words from the raw stage and splits them
 // there, so the MMA warps do nothing but load, split and issue in the K loop.  setmaxnreg gives the producer
-// warpgroup 40 registers per thread and the consumers 232.
+// warpgroup 40 registers per thread and the consumers 232.  Its CTAs are persistent (one wave, a static task list per
+// CTA): the producer warps run ahead into the next task, and the epilogue works straight from the accumulator
+// registers.
 #pragma once
 
 #include <cuda.h>
@@ -771,7 +773,65 @@ constexpr int X3_STAGE_BYTES = TC_STAGE_BYTES + TC_B_BYTES;   // [A raw | B raw 
 constexpr int X3_CHUNK = 8;                                   // slabs (256 K columns) per tensor-core accumulation
 static_assert(X3_CHUNK % 2 == 0, "the A fragment register sets alternate by slab within a chunk");
 constexpr int x3_smem_bytes() { return X3_STAGES * X3_STAGE_BYTES + 1024; }
-static_assert(TC_ACC_BYTES <= X3_STAGES * X3_STAGE_BYTES, "the precise kernel reuses its operand ring");
+
+// Static schedule of a launch: CTA b runs the tasks (linear tile numbers, split included) task[off[b] .. off[b+1]),
+// longest first, as assigned by the LPT model of the split planner (x3_makespan).  A launch with more tasks than the
+// list holds runs them strided instead (task = blockIdx.x + i * gridDim.x).
+constexpr int kX3MaxCtas = 144;
+constexpr int kX3MaxTasks = 1024;
+struct X3Sched {
+  int listed;                                   // 1: the lists below; 0: strided
+  unsigned short off[kX3MaxCtas + 1];
+  unsigned short task[kX3MaxTasks];
+};
+static_assert(sizeof(GemmTable) + sizeof(TcMaps) + sizeof(TcSegMaps) + sizeof(X3Sched) + 256 <= 32764,
+              "kernel parameters of the precise kernel exceed the 32 KB limit");
+
+// One task as the roles read it: the group and segments (TileCtx), and where the task sits in it.  Two slots: the
+// producer warp stages task k + 1 while the consumers still run the epilogue of task k.
+struct X3Slot {
+  TileCtx ctx;
+  int split, m0, n0, c_begin, n_iter;
+};
+// readers that release a slot: the 8 consumer warps (after the epilogue) and the 3 split warps
+constexpr int X3_SLOT_READERS = TC_CONSUMER_WARPS + 3;
+
+__device__ __forceinline__ int x3_task(const X3Sched& sched, const int k) {
+  return sched.listed ? (int)sched.task[sched.off[blockIdx.x] + k] : (int)(blockIdx.x + k * gridDim.x);
+}
+
+// Stage task `tile` into slot `sl` (one whole warp; parameter space and shared memory only).
+__device__ __forceinline__ void x3_stage(const GemmTable& tab, const TcSegMaps& sm, const int tile, X3Slot* sl) {
+  const int lane = threadIdx.x & 31;
+  int best = 0;
+  for (int i = lane; i < tab.n_groups; i += 32)
+    if (tile >= tab.g[i].tile_begin) best = max(best, i);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
+  const int* src = reinterpret_cast<const int*>(&tab.g[best]);
+  int* dst = reinterpret_cast<int*>(&sl->ctx.g);
+  for (int i = lane; i < (int)(sizeof(Group) / sizeof(int)); i += 32) dst[i] = src[i];
+  const int sb = tab.g[best].seg_begin, sc = tab.g[best].seg_count;
+  for (int i = lane; i < sc; i += 32) {
+    const Seg& s = tab.s[sb + i];
+    SegLite l;
+    l.A = s.A;
+    l.B = s.B;
+    l.len = s.len;
+    l.lda = s.lda;
+    l.ldb = s.ldb;
+    l.amap = sm.a[sb + i];
+    l.bmap = sm.b[sb + i];
+    sl->ctx.seg[i] = l;
+  }
+  __syncwarp();
+  if (lane == 0) {
+    sl->ctx.gi = best;
+    tc_decode(sl->ctx, tile, &sl->split, &sl->m0, &sl->n0);
+    tc_chunk_range(sl->ctx, sl->split, &sl->c_begin, &sl->n_iter);
+  }
+  __syncwarp();
+}
 
 // the 96 split threads only
 __device__ __forceinline__ void x3_split_sync() { asm volatile("bar.sync 2, 96;" ::: "memory"); }
@@ -836,14 +896,15 @@ __device__ __forceinline__ void x3_load_a(const uint32_t a_raw, const uint32_t o
   }
 }
 
-// Consumer warpgroups: slab `it` of the tile.  The fragments (hi, lo) must not belong to the group still in flight:
-// the caller alternates two register sets.  Leaves this slab's group in flight and releases the previous stage.
+// Consumer warpgroups: slab `gl` of the CTA (running count over its tasks).  The fragments (hi, lo) must not belong to
+// the group still in flight: the caller alternates two register sets.  Leaves this slab's group in flight and releases
+// the previous stage.
 template <bool A_KMAJ>
-__device__ __forceinline__ void x3_consume_slab(const int it, uint8_t* smem, TcShared* sh, uint64_t* ready_bar,
+__device__ __forceinline__ void x3_consume_slab(const uint32_t gl, uint8_t* smem, TcShared* sh, uint64_t* ready_bar,
                                                 const uint32_t off0, const uint32_t off1, uint32_t (&hi)[16],
                                                 uint32_t (&lo)[16], float (&d)[64], int& prev) {
-  const int stage = it % X3_STAGES;
-  const uint32_t parity = (uint32_t)(it / X3_STAGES) & 1u;
+  const int stage = (int)(gl % X3_STAGES);
+  const uint32_t parity = (gl / X3_STAGES) & 1u;
   mbar_wait(&sh->full_bar[stage], parity);          // raw A landed (read below with ordinary loads)
   mbar_wait(&ready_bar[stage], parity);             // B lo (and transposed MN-major B) written
   const uint32_t a_raw = smem_u32(smem + stage * X3_STAGE_BYTES);
@@ -866,85 +927,217 @@ __device__ __forceinline__ void x3_consume_slab(const int it, uint8_t* smem, TcS
   prev = stage;
 }
 
+// ---- epilogue straight from the accumulator fragment (consumer thread) ------------------------------------------
+// Thread (warp w, lane l) holds rows r0 = 64 (w / 4) + 16 (w % 4) + l / 4 and r0 + 8 of the tile, columns
+// 8j + 2(l % 4) + {0, 1} (see wgmma_tf32): v[4j + 2h + e] = (row r0 + 8h, column c0 + 8j + e), c0 = 2(l % 4).  A warp
+// store instruction then covers 8 rows x 32 B, whole sectors.
+__device__ __forceinline__ void x3_st2(float* p, const float x0, const float x1, const bool vec, const bool two) {
+  if (vec) {
+    *reinterpret_cast<float2*>(p) = make_float2(x0, x1);
+  } else {
+    p[0] = x0;
+    if (two) p[1] = x1;
+  }
+}
+
+// The fused epilogue of the fragment -> C.  The forward flag sets (bias, ReLU, RNG dropout) work from register copies
+// of the group fields and draw one rng_hash4 per 4-column group; every other set applies epilogue_t per element.
+template <int F>
+__device__ __forceinline__ void x3_epilogue(const Group& g, const int m0, const int n0, const float (&v)[64]) {
+  constexpr bool kFwd = F >= 0 && (F & ~(EPI_BIAS | EPI_RELU | EPI_DROP_RNG)) == 0;
+  const int M = g.M, N = g.N, ldc = g.ldc;
+  float* const C = g.C;
+  const bool vec = (N % 2) == 0 && (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) & 7u) == 0;
+  const float alpha = kFwd ? (g.alpha_dev ? g.alpha * __ldg(g.alpha_dev) : g.alpha) : 0.f;
+  const float* const bias = g.bias;
+  const uint64_t seed = g.seed, roff = g.rng_offset;
+  const uint64_t step = (kFwd && (F & EPI_DROP_RNG) && g.step_dev) ? *g.step_dev : 0ull;
+  const float dscale = g.drop_scale, dp = g.drop_p;
+  const uint32_t thr = rng_threshold(dp);
+  float b0[16], b1[16];                 // bias of the thread's columns, loaded before the first store
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int n = n0 + 8 * j;
+    b0[j] = kFwd && (F & EPI_BIAS) && n < N ? bias[n] : 0.f;
+    b1[j] = kFwd && (F & EPI_BIAS) && n + 1 < N ? bias[n + 1] : 0.f;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = m0 + 8 * h;
+    if (m >= M) continue;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int n = n0 + 8 * j;
+      if (n >= N) continue;
+      const bool two = n + 1 < N;
+      float x0 = v[4 * j + 2 * h], x1 = v[4 * j + 2 * h + 1];
+      if (kFwd) {
+        x0 *= alpha;
+        x1 *= alpha;
+        if (F & EPI_BIAS) {
+          x0 += b0[j];
+          x1 += b1[j];
+        }
+        if (F & EPI_RELU) {
+          x0 = fmaxf(x0, 0.0f);
+          x1 = fmaxf(x1, 0.0f);
+        }
+        if (F & EPI_DROP_RNG) {
+          const uint64_t e = roff + (uint64_t)m * (uint64_t)N + (uint64_t)n;
+          bool k0, k1;
+          if ((e & 1ull) == 0) {        // the pair lies in one 4-column group of the RNG stream
+            const uint64_t hsh = rng_hash4(seed, step, e >> 2);
+            k0 = rng_keep_bits(hsh, (int)(e & 3ull), thr);
+            k1 = rng_keep_bits(hsh, (int)(e & 3ull) + 1, thr);
+          } else {
+            k0 = rng_keep(seed, step, e, dp);
+            k1 = rng_keep(seed, step, e + 1, dp);
+          }
+          const float f0 = k0 ? dscale : 0.0f, f1 = k1 ? dscale : 0.0f;
+          x0 = f0 != 0.0f ? x0 * f0 : 0.0f;
+          x1 = f1 != 0.0f ? x1 * f1 : 0.0f;
+        }
+      } else {
+        x0 = epilogue_t<F>(g, m, n, x0);
+        if (two) x1 = epilogue_t<F>(g, m, n + 1, x1);
+      }
+      x3_st2(C + (size_t)m * ldc + n, x0, x1, vec, two);
+    }
+  }
+}
+
+// The finished task (all 256 consumer threads).  Unsplit: epilogue -> C.  Split: raw partial -> partial[split] (the
+// separate fixed-order reduce pass applies the epilogue).
+__device__ __forceinline__ void x3_finish(const X3Slot& sl, const float (&v)[64]) {
+  const Group& g = sl.ctx.g;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m0 = sl.m0 + (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2), n0 = sl.n0 + 2 * (lane & 3);
+  if (g.ksplit > 1) {
+    const int M = g.M, N = g.N;
+    float* const part = g.partial + (size_t)sl.split * M * N;
+    const bool vec = (N % 2) == 0;          // partial planes are 256-B aligned
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int m = m0 + 8 * h, n = n0 + 8 * j;
+        if (m < M && n < N) x3_st2(part + (size_t)m * N + n, v[4 * j + 2 * h], v[4 * j + 2 * h + 1], vec, n + 1 < N);
+      }
+    return;
+  }
+  TA3N_EPI_DISPATCH(g.flags, { x3_epilogue<EPI_F>(g, m0, n0, v); })
+}
+
 template <bool A_KMAJ, bool B_KMAJ>
 __global__ void __launch_bounds__(X3_THREADS, 1)
 seg_gemm_tc_x3_kernel(const __grid_constant__ GemmTable tab, const __grid_constant__ TcMaps maps,
-                      const __grid_constant__ TcSegMaps segmaps) {
+                      const __grid_constant__ TcSegMaps segmaps, const __grid_constant__ X3Sched sched) {
   extern __shared__ uint8_t tc_smem_raw[];
   __shared__ __align__(8) TcShared sh;
   __shared__ __align__(8) uint64_t ready_bar[X3_STAGES];     // B split done (one arrival per split warp)
-  __shared__ TileCtx ctx;
+  __shared__ __align__(8) uint64_t slot_full[2], slot_empty[2];
+  __shared__ X3Slot slots[2];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // every CTA has at least one task (the grid is no larger than the task count)
+  const int n_tasks = sched.listed ? sched.off[blockIdx.x + 1] - sched.off[blockIdx.x]
+                                   : (tab.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
-  const int tile = blockIdx.x;
-  load_tile_ctx(tab, tile, &ctx, segmaps.a, segmaps.b);
-  int split, m0, n0, c_begin, n_iter;
-  tc_decode(ctx, tile, &split, &m0, &n0);
-  tc_chunk_range(ctx, split, &c_begin, &n_iter);
-
-  if (warp == TC_CONSUMER_WARPS && lane == 0) {
-    for (int s = 0; s < X3_STAGES; ++s) mbar_init(&ready_bar[s], X3_SPLIT_WARPS);
-    tc_pipe_init<X3_STAGES>(&sh);
+  if (warp == TC_CONSUMER_WARPS) {
+    if (lane == 0) {
+      for (int s = 0; s < X3_STAGES; ++s) mbar_init(&ready_bar[s], X3_SPLIT_WARPS);
+      for (int s = 0; s < 2; ++s) {
+        mbar_init(&slot_full[s], 1);
+        mbar_init(&slot_empty[s], X3_SLOT_READERS);
+      }
+      tc_pipe_init<X3_STAGES>(&sh);
+    }
+    __syncwarp();
+    x3_stage(tab, segmaps, x3_task(sched, 0), &slots[0]);
+    if (lane == 0) mbar_arrive(&slot_full[0]);
   }
   __syncthreads();
+  // Everything above touched only kernel parameters and shared memory: it overlaps the previous kernel of the
+  // stream.  From here on operands produced by that kernel are read.
   pdl_wait();
 
   if (warp >= TC_CONSUMER_WARPS) {
     setmaxnreg_dec<X3_PRODUCER_REGS>();
+    uint32_t slabs = 0;                 // slabs of the CTA so far: ring stage and parity
     if (warp == TC_CONSUMER_WARPS) {
-      if (lane == 0 && n_iter > 0)
-        tc_produce<X3_STAGES, X3_STAGE_BYTES>(ctx, maps.m, A_KMAJ, B_KMAJ, tab.pad_, m0, n0, c_begin, n_iter, smem, &sh,
-                                              0u);
+      for (int k = 0; k < n_tasks; ++k) {
+        const int s = k & 1;
+        if (k > 0) {                    // stage task k once the epilogue of task k - 2 has left the slot
+          mbar_wait(&slot_empty[s], ((uint32_t)(k >> 1) & 1u) ^ 1u);
+          x3_stage(tab, segmaps, x3_task(sched, k), &slots[s]);
+          if (lane == 0) mbar_arrive(&slot_full[s]);
+        }
+        const X3Slot& sl = slots[s];
+        if (lane == 0 && sl.n_iter > 0)
+          tc_produce<X3_STAGES, X3_STAGE_BYTES>(sl.ctx, maps.m, A_KMAJ, B_KMAJ, tab.pad_, sl.m0, sl.n0, sl.c_begin,
+                                                sl.n_iter, smem, &sh, slabs);
+        __syncwarp();
+        slabs += (uint32_t)sl.n_iter;
+      }
     } else {
       const int t = threadIdx.x - 32 * (TC_CONSUMER_WARPS + 1);
-      for (int it = 0; it < n_iter; ++it) {
-        const int stage = it % X3_STAGES;
-        mbar_wait(&sh.full_bar[stage], (uint32_t)(it / X3_STAGES) & 1u);
-        const uint32_t b_raw = smem_u32(smem + stage * X3_STAGE_BYTES) + TC_A_BYTES;
-        x3_split_b<B_KMAJ>(b_raw, b_raw + TC_B_BYTES, t);
-        fence_proxy_async();            // generic-proxy writes -> the tensor core's reads
+      for (int k = 0; k < n_tasks; ++k) {
+        const int s = k & 1;
+        mbar_wait(&slot_full[s], (uint32_t)(k >> 1) & 1u);
+        const int n_iter = slots[s].n_iter;
         __syncwarp();
-        if (lane == 0) mbar_arrive(&ready_bar[stage]);
+        if (lane == 0) mbar_arrive(&slot_empty[s]);
+        for (int it = 0; it < n_iter; ++it) {
+          const uint32_t gl = slabs + (uint32_t)it;
+          const int stage = (int)(gl % X3_STAGES);
+          mbar_wait(&sh.full_bar[stage], (gl / X3_STAGES) & 1u);
+          const uint32_t b_raw = smem_u32(smem + stage * X3_STAGE_BYTES) + TC_A_BYTES;
+          x3_split_b<B_KMAJ>(b_raw, b_raw + TC_B_BYTES, t);
+          fence_proxy_async();          // generic-proxy writes -> the tensor core's reads
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&ready_bar[stage]);
+        }
+        slabs += (uint32_t)n_iter;
       }
     }
   } else {
     setmaxnreg_inc<X3_CONSUMER_REGS>();
     const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);      // fragment rows r0, r0 + 8
     const uint32_t off0 = x3_a_thread_off<A_KMAJ>(r0, lane & 3), off1 = x3_a_thread_off<A_KMAJ>(r0 + 8, lane & 3);
-    float d[64], sum[64];
+    uint32_t slabs = 0;
+    for (int k = 0; k < n_tasks; ++k) {
+      const int s = k & 1;
+      mbar_wait(&slot_full[s], (uint32_t)(k >> 1) & 1u);
+      const int n_iter = slots[s].n_iter;
+      float d[64], sum[64];
 #pragma unroll
-    for (int j = 0; j < 64; ++j) d[j] = sum[j] = 0.f;
-    uint32_t hi[2][16], lo[2][16];      // A fragments of the even / odd slabs of a chunk
-    // One group of MMAs stays in flight while the next slab's fragments are loaded; at the end of a chunk every MMA
-    // must have finished before the fold reads the accumulator.
-    int prev = -1;                      // stage whose MMAs may still be in flight
-    for (int c0 = 0; c0 < n_iter; c0 += X3_CHUNK) {
-      const int c1 = min(n_iter, c0 + X3_CHUNK);
-      for (int it = c0; it < c1; it += 2) {
-        x3_consume_slab<A_KMAJ>(it, smem, &sh, ready_bar, off0, off1, hi[0], lo[0], d, prev);
-        if (it + 1 < c1) x3_consume_slab<A_KMAJ>(it + 1, smem, &sh, ready_bar, off0, off1, hi[1], lo[1], d, prev);
+      for (int j = 0; j < 64; ++j) d[j] = sum[j] = 0.f;
+      uint32_t hi[2][16], lo[2][16];    // A fragments of the even / odd slabs of a chunk
+      // One group of MMAs stays in flight while the next slab's fragments are loaded; at the end of a chunk every MMA
+      // must have finished before the fold reads the accumulator.
+      int prev = -1;                    // stage whose MMAs may still be in flight
+      for (int c0 = 0; c0 < n_iter; c0 += X3_CHUNK) {
+        const int c1 = min(n_iter, c0 + X3_CHUNK);
+        for (int it = c0; it < c1; it += 2) {
+          x3_consume_slab<A_KMAJ>(slabs + (uint32_t)it, smem, &sh, ready_bar, off0, off1, hi[0], lo[0], d, prev);
+          if (it + 1 < c1)
+            x3_consume_slab<A_KMAJ>(slabs + (uint32_t)(it + 1), smem, &sh, ready_bar, off0, off1, hi[1], lo[1], d, prev);
+        }
+        wgmma_wait<0>();                // chunk complete: fold it into the fp32 sums
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&sh.empty_bar[prev]);
+        prev = -1;
+#pragma unroll
+        for (int j = 0; j < 64; ++j) {
+          sum[j] += d[j];
+          d[j] = 0.f;
+        }
       }
-      wgmma_wait<0>();                  // chunk complete: fold it into the fp32 sums
+      slabs += (uint32_t)n_iter;
+      x3_finish(slots[s], sum);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&sh.empty_bar[prev]);
-      prev = -1;
-#pragma unroll
-      for (int j = 0; j < 64; ++j) {
-        sum[j] += d[j];
-        d[j] = 0.f;
-      }
+      if (lane == 0) mbar_arrive(&slot_empty[s]);
     }
-    consumer_sync();                    // every MMA has read the ring: it becomes the accumulator tile
-    float* acc = reinterpret_cast<float*>(smem);
-    tc_store_acc(acc, sum, threadIdx.x);
-    consumer_sync();
-    // the tile coordinates again from the staged context: kept live across the K loop they cost registers there
-    int e_split, e_m0, e_n0, e_begin, e_iter;
-    tc_decode(ctx, tile, &e_split, &e_m0, &e_n0);
-    tc_chunk_range(ctx, e_split, &e_begin, &e_iter);
-    tc_epilogue<TC_CONSUMER_WARPS>(ctx, e_m0, e_n0, e_split, e_iter, ctx.g.ksplit > 1 ? TILE_PARTIAL : TILE_FINAL, acc,
-                                   warp);
   }
 }
 
@@ -1090,7 +1283,8 @@ inline int tc_launch_one(const GemmTable& tab, const TcMaps& maps, const TcSegMa
 
 // the precise kernel, per operand layout
 template <bool A_KMAJ, bool B_KMAJ>
-inline int tc_launch_x3(const GemmTable& tab, const TcMaps& maps, const TcSegMaps& sm, cudaStream_t stream, const char* label) {
+inline int tc_launch_x3(const GemmTable& tab, const TcMaps& maps, const TcSegMaps& sm, const X3Sched& sched, int grid,
+                        cudaStream_t stream, const char* label) {
   constexpr int slot = (A_KMAJ ? 0 : 1) + (B_KMAJ ? 0 : 2);
   {
     std::lock_guard<std::mutex> lock(device_mu());
@@ -1103,7 +1297,7 @@ inline int tc_launch_x3(const GemmTable& tab, const TcMaps& maps, const TcSegMap
     }
   }
   pre_launch(label, stream);
-  launch_kernel(seg_gemm_tc_x3_kernel<A_KMAJ, B_KMAJ>, tab.total_tiles, X3_THREADS, x3_smem_bytes(), stream, tab, maps, sm);
+  launch_kernel(seg_gemm_tc_x3_kernel<A_KMAJ, B_KMAJ>, grid, X3_THREADS, x3_smem_bytes(), stream, tab, maps, sm, sched);
   return after_launch();
 }
 
@@ -1134,6 +1328,35 @@ inline void tc_rank3_flags(const GemmPlan& plan, bool* a3d, bool* b3d) {
   }
 }
 
+inline double x3_makespan(const GemmPlan& plan, const std::vector<int>& ks, int sms,
+                          std::vector<std::vector<std::pair<int, int>>>* assign = nullptr);
+
+// The precise kernel's schedule for the groups [g_first, g_first + tab.n_groups) of `plan` staged in `tab`: the LPT
+// lists of x3_makespan, one CTA per non-empty list.  Returns the grid size.
+inline int x3_schedule(const GemmPlan& plan, size_t g_first, const GemmTable& tab, X3Sched* sched) {
+  const int ctas = std::min(device_sm_count(), kX3MaxCtas);
+  if (tab.total_tiles > kX3MaxTasks) {
+    sched->listed = 0;
+    return std::min(tab.total_tiles, ctas);
+  }
+  std::vector<int> idx, ks;
+  for (int i = 0; i < tab.n_groups; ++i) {
+    idx.push_back((int)g_first + i);
+    ks.push_back(tab.g[i].ksplit);
+  }
+  std::vector<std::vector<std::pair<int, int>>> lists;
+  x3_makespan(sub_plan(plan, idx), ks, ctas, &lists);
+  sched->listed = 1;
+  int grid = 0, n = 0;
+  for (const auto& l : lists) {
+    if (l.empty()) continue;
+    sched->off[grid++] = (unsigned short)n;
+    for (const auto& gt : l) sched->task[n++] = (unsigned short)(tab.g[gt.first].tile_begin + gt.second);
+  }
+  sched->off[grid] = (unsigned short)n;
+  return grid;
+}
+
 // Launch `plan` (all groups eligible) on the tensor-core engine.
 inline int launch_tc(const GemmPlan& plan_in, cudaStream_t stream, bool precise = false) {
   // longest-K groups first (see the tile remap in the kernel): LPT-style balance of the tensor pipe
@@ -1148,6 +1371,7 @@ inline int launch_tc(const GemmPlan& plan_in, cudaStream_t stream, bool precise 
   tc_rank3_flags(plan, &a3d, &b3d);
   size_t gi = 0;
   while (gi < plan.groups.size()) {
+    const size_t g_first = gi;
     GemmTable tab;
     TcMaps maps;
     TcSegMaps sm;
@@ -1201,14 +1425,16 @@ inline int launch_tc(const GemmPlan& plan_in, cudaStream_t stream, bool precise 
     tab.total_tiles = tiles;
     tab.pad_ = (a3d ? 1 : 0) | (b3d ? 2 : 0);
     if (tiles > 0) {
+      X3Sched sched;
+      const int grid = precise ? x3_schedule(plan, g_first, tab, &sched) : 0;
       if (precise && plan.a_kmaj && plan.b_kmaj)
-        TA3N_TRY((tc_launch_x3<true, true>(tab, maps, sm, stream, plan.label)));
+        TA3N_TRY((tc_launch_x3<true, true>(tab, maps, sm, sched, grid, stream, plan.label)));
       else if (precise && plan.a_kmaj && !plan.b_kmaj)
-        TA3N_TRY((tc_launch_x3<true, false>(tab, maps, sm, stream, plan.label)));
+        TA3N_TRY((tc_launch_x3<true, false>(tab, maps, sm, sched, grid, stream, plan.label)));
       else if (precise && !plan.a_kmaj && !plan.b_kmaj)
-        TA3N_TRY((tc_launch_x3<false, false>(tab, maps, sm, stream, plan.label)));
+        TA3N_TRY((tc_launch_x3<false, false>(tab, maps, sm, sched, grid, stream, plan.label)));
       else if (precise)
-        TA3N_TRY((tc_launch_x3<false, true>(tab, maps, sm, stream, plan.label)));
+        TA3N_TRY((tc_launch_x3<false, true>(tab, maps, sm, sched, grid, stream, plan.label)));
       else if (plan.a_kmaj && plan.b_kmaj)
         TA3N_TRY((tc_launch_one<true, true>(tab, maps, sm, stream, plan.label)));
       else if (plan.a_kmaj && !plan.b_kmaj)
@@ -1268,17 +1494,32 @@ inline int x3_plan_slabs(const GemmPlan& plan, const Group& g) {
   for (int k = 0; k < g.seg_count; ++k) n += (plan.segs[g.seg_begin + k].len + TC_BK - 1) / TC_BK;
   return n;
 }
-inline double x3_makespan(const GemmPlan& plan, const std::vector<int>& ks, int sms) {
-  std::vector<double> tasks;
+// Greedy (LPT) assignment of the tasks of `plan` (group gi split ks[gi] ways: tiles * ks[gi] tasks, numbered within the
+// group) to `sms` SMs; returns the makespan.  `assign`, when given, receives the task list of each SM as (group, task)
+// pairs, longest first: the precise kernel runs exactly this schedule.
+inline double x3_makespan(const GemmPlan& plan, const std::vector<int>& ks, int sms,
+                          std::vector<std::vector<std::pair<int, int>>>* assign) {
+  struct Task {
+    double len;
+    int g, t;
+  };
+  std::vector<Task> tasks;
   for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
     const Group& g = plan.groups[gi];
     const int tiles = ((g.M + TC_BM - 1) / TC_BM) * ((g.N + TC_BN - 1) / TC_BN);
     const double len = (double)x3_plan_slabs(plan, g) / ks[gi] + 4.0;      // + prologue / epilogue, in slab units
-    for (int t = 0; t < tiles * ks[gi]; ++t) tasks.push_back(len);
+    for (int t = 0; t < tiles * ks[gi]; ++t) tasks.push_back({len, (int)gi, t});
   }
-  std::sort(tasks.begin(), tasks.end(), std::greater<double>());
+  std::sort(tasks.begin(), tasks.end(), [](const Task& a, const Task& b) {
+    return a.len != b.len ? a.len > b.len : std::tie(a.g, a.t) < std::tie(b.g, b.t);
+  });
   std::vector<double> load(sms, 0.0);
-  for (double t : tasks) *std::min_element(load.begin(), load.end()) += t;
+  if (assign) assign->assign(sms, {});
+  for (const Task& t : tasks) {
+    const auto it = std::min_element(load.begin(), load.end());
+    *it += t.len;
+    if (assign) (*assign)[it - load.begin()].push_back({t.g, t.t});
+  }
   return *std::max_element(load.begin(), load.end());
 }
 inline void plan_splitk_balanced(GemmPlan& plan, Arena* arena, int sms) {
