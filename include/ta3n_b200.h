@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define TA3N_ABI_VERSION 2
+#define TA3N_ABI_VERSION 3
 
 enum {
   TA3N_OK = 0,
@@ -255,20 +255,15 @@ int ta3n_loss_fwd_bwd(const float* pred_video, const long long* labels, const fl
 /* *counter += 1 on the stream (dropout step counter for CUDA-graph replays). */
 int ta3n_counter_inc(uint64_t* counter, ta3n_stream_t stream);
 
-/* ---- the fused training step (SURVEY 8a rows a1-a13 + 8f row n1 in one launch) ---------------------------- */
+/* ---- the training step as one step program (SURVEY 8a rows a1-a13 + 8f row n1) ----------------------------- */
 /* main.py:418 (model forward, models.py:545-722 trn-m branch), main.py:446, 508-538, 559-562 (composed loss:
  * class CE + domain CE per adversarial level + gamma * attentive entropy, loss.py:15-25) and main.py:576
  * (backward to every parameter gradient) for one paired mini-batch, use_attn_frame == 'none'.
  *
- * Everything is described once by a ta3n_step_desc (device pointers unless noted).  Two executors give
- * bit-identical results:
- *   ta3n_step_run_phased : one launch per dependency level -- 8 grouped GEMM launches (engine as selected), 4 row
- *                          kernels (frame rows; per video: relation pooling, loss heads, relation backward) and
- *                          2 column-sum launches (14 launches; the round-1 sequence had 25);
- *   ta3n_step_build + ta3n_step_run : the same work as ONE persistent kernel (one CTA per SM) whose CTAs claim
- *                          READY GEMM tiles / row tasks / column-sum tasks from priority queues and synchronise
- *                          through arrival counters in global memory (csrc/step_kernel.cuh) -- plus one memset node.
- * Both are CUDA-graph capturable (ta3n_step_build itself is not: it copies the task graph to the device).        */
+ * Everything is described once by a ta3n_step_desc (device pointers unless noted).  ta3n_step_run_phased enqueues
+ * one launch per dependency level: 8 grouped GEMM launches (engine as selected), 4 row kernels (frame rows; per
+ * video: relation pooling, loss heads, relation backward) and 2 column-sum launches (14 launches; the round-1
+ * sequence had 25).  It is CUDA-graph capturable.                                                                 */
 typedef struct {
   int Bs, Bt;                 /* source / target videos of the mini-batch (M = Bs + Bt rows, source first)         */
   int T, D, F, H, C;          /* frames per video, input width, shared width (fc_dim), bottleneck (256), classes    */
@@ -325,24 +320,10 @@ typedef struct {
   size_t workspace_bytes;
 } ta3n_step_desc;
 
-#define TA3N_STEP_HANDLE_BYTES 256
+/* Bytes of desc->workspace: the fixed scratch tensors plus the column sums' partials.  Pointers in desc only need to
+ * be non-null; no CUDA call.  0 on an invalid descriptor (ta3n_last_error() says why).                              */
 size_t ta3n_step_workspace_bytes(const ta3n_step_desc* desc);
 int ta3n_step_run_phased(const ta3n_step_desc* desc, ta3n_stream_t stream);
-size_t ta3n_step_plan_bytes(const ta3n_step_desc* desc);
-/* Builds the task graph for `desc` (pointers are baked in) into plan_dev (device, ta3n_step_plan_bytes(desc) bytes;
- * synchronous copy) and fills handle_host (HOST memory, TA3N_STEP_HANDLE_BYTES bytes) for ta3n_step_run.           */
-int ta3n_step_build(const ta3n_step_desc* desc, void* plan_dev, size_t plan_bytes, void* handle_host);
-int ta3n_step_run(const void* handle_host, ta3n_stream_t stream);
-/* Host-only summary of the task graph of `desc` (counts per task type, arrival counters, K slabs, and the number of
- * tasks a simulated scheduler can never run -- must be 0: the dependency graph is acyclic and every awaited count is
- * reached).  No CUDA call.                                                                                          */
-size_t ta3n_step_describe(const ta3n_step_desc* desc, char* buf, size_t buf_bytes);
-/* Optional per-task trace: trace_dev (device, n_tasks * 8 uint64) receives {SM id | tag, started, accumulator ready,
- * done, body done, CTA synced, 0, 0} (globaltimer ns) of every task of the following runs; NULL switches it off.
- * tools/step_trace.py reads it.                                                                                     */
-int ta3n_step_set_trace(void* handle_host, unsigned long long* trace_dev);
-/* number of tasks / arrival counters of a built plan (diagnostics) */
-int ta3n_step_info(const void* handle_host, int* n_tasks, int* n_counters, int* n_gemm_tiles);
 
 /* ---- gradient all-reduce over NVLink / NVSwitch peer memory (SURVEY 8e; replaces nn.DataParallel's reduce, main.py:79) */
 /* In-place MEAN over the `world` ranks of one node of n floats (n % 4 == 0) that live at the same offset of a symmetric,

@@ -11,6 +11,8 @@ import threading
 
 from . import build as _build
 
+ABI_VERSION = 3      # TA3N_ABI_VERSION of include/ta3n_b200.h that SIGNATURES mirrors
+
 TA3N_GEMM_FP32_SIMT = 0
 TA3N_GEMM_TF32_TCGEN05 = 1
 TA3N_GEMM_TF32X3_TCGEN05 = 2
@@ -47,8 +49,6 @@ class StepDesc(C.Structure):
                                    "step_counter", "workspace")] +
         [("workspace_bytes", C.c_size_t)])
 
-
-STEP_HANDLE_BYTES = 256
 
 _VP, _I, _F, _SZ = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _IP = C.POINTER(C.c_int)
@@ -104,12 +104,6 @@ SIGNATURES = {
     "ta3n_counter_inc": (_I, [_VP, _VP]),
     "ta3n_step_workspace_bytes": (_SZ, [C.POINTER(StepDesc)]),
     "ta3n_step_run_phased": (_I, [C.POINTER(StepDesc), _VP]),
-    "ta3n_step_plan_bytes": (_SZ, [C.POINTER(StepDesc)]),
-    "ta3n_step_build": (_I, [C.POINTER(StepDesc), _VP, _SZ, _VP]),
-    "ta3n_step_run": (_I, [_VP, _VP]),
-    "ta3n_step_describe": (_SZ, [C.POINTER(StepDesc), C.c_char_p, _SZ]),
-    "ta3n_step_set_trace": (_I, [_VP, _VP]),
-    "ta3n_step_info": (_I, [_VP, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "ta3n_allreduce_flag_bytes": (_SZ, [_I]),
     "ta3n_allreduce_mean": (_I, [_PP, _VP, _PP, _VP, _I, _I, C.c_longlong, _VP]),
     "ta3n_sgd_workspace_bytes": (_SZ, []),
@@ -148,7 +142,7 @@ def load() -> C.CDLL:
                 fn = getattr(lib, name)   # AttributeError if the .so does not export the symbol
                 fn.restype = res
                 fn.argtypes = args
-            if lib.ta3n_abi_version() != 2:
+            if lib.ta3n_abi_version() != ABI_VERSION:
                 raise Ta3nError("libta3n_sm90.so ABI version mismatch")
             _lib = lib
     return _lib

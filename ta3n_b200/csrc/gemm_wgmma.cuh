@@ -93,7 +93,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// the 256 consumer threads (warps 0..7) only; the same named barrier as row_sync() of the step kernel's row tasks
+// the 256 consumer threads (warps 0..7) only
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
@@ -254,10 +254,9 @@ __device__ __forceinline__ void acc_ld_32(const float* acc, int row, int col0, f
 }
 
 // ---- one output tile, by warp role ---------------------------------------------------------------------
-// Shared by the per-launch kernels below (one tile per CTA) and by the persistent step kernel (step_kernel.cuh), where
-// the producer runs ahead over the task queue: it fills the ring with the slabs of tile t+1 while the consumer warps
-// still finish tile t.  The operand ring barriers are initialised once per CTA; each role keeps its own running slab
-// count.
+// The operand ring barriers are initialised once per CTA.  The precise kernel's producer runs ahead over its task
+// list (it fills the ring with the slabs of task t+1 while the consumer warps still finish task t), so it passes its
+// running slab count to tc_produce.
 struct TcShared {
   uint64_t full_bar[4];      // TMA landed
   uint64_t empty_bar[4];     // every consumer warp is done with the stage
@@ -274,13 +273,8 @@ __device__ __forceinline__ void tc_pipe_init(TcShared* sh) {
 
 // What a tile of a split-K group does with its accumulator:
 //   TILE_FINAL   : fused epilogue -> C                       (ksplit == 1)
-//   TILE_PARTIAL : raw accumulator -> partial[split]         (separate reduce pass, or an owner tile below)
-//   TILE_OWNER   : adds partial[0 .. ksplit-2] in a fixed order, then fused epilogue -> C.  The caller guarantees
-//                  those partials are complete and visible (step kernel: task dependency).
-//   TILE_SPLIT   : (step kernel) raw accumulator -> partial[split]; the LAST split of the tile to arrive (arrival counter)
-//                  then runs a TILE_REDUCE pass: partial[0 .. ksplit-1] summed in split order + fused epilogue -> C.
-//                  No split ever waits for another one, and the result does not depend on which one came last.
-enum : int { TILE_FINAL = 0, TILE_PARTIAL = 1, TILE_OWNER = 2, TILE_SPLIT = 3, TILE_REDUCE = 4 };
+//   TILE_PARTIAL : raw accumulator -> partial[split]         (a separate reduce pass applies the epilogue)
+enum : int { TILE_FINAL = 0, TILE_PARTIAL = 1 };
 
 // TMA producer (ONE thread): the n_iter K slabs [c_begin, c_begin + n_iter) of tile (m0, n0) into the ring.
 // `slabs` = slabs this CTA has pushed so far (advanced by the caller).
@@ -344,13 +338,13 @@ __device__ __forceinline__ void tc_produce(const TileCtx& ctx, const CUtensorMap
 // 64 wg .. 64 wg + 63).  One group of MMAs stays in flight while the next stage is prepared.
 template <int STAGES>
 __device__ __forceinline__ void tc_consume(const bool a_kmaj, const bool b_kmaj, const int n_iter, uint8_t* smem,
-                                           TcShared* sh, const uint32_t slabs, float (&d)[64]) {
+                                           TcShared* sh, float (&d)[64]) {
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
 #pragma unroll
   for (int j = 0; j < 64; ++j) d[j] = 0.f;
   int prev = -1;
   for (int it = 0; it < n_iter; ++it) {
-    const uint32_t gl = slabs + (uint32_t)it;
+    const uint32_t gl = (uint32_t)it;
     const int stage = (int)(gl % STAGES);
     mbar_wait(&sh->full_bar[stage], (gl / STAGES) & 1u);
     const uint32_t a_base = smem_u32(smem + stage * TC_STAGE_BYTES);
@@ -402,22 +396,6 @@ __device__ __forceinline__ void tc_epilogue(const TileCtx& ctx, const int m0, co
     if (m < e.M && nb < e.N) {
       float* orow = obase + (size_t)m * ldo + nb;
       const int nvalid = min(32, e.N - nb);
-      if (mode == TILE_OWNER) {      // raw partial sums of the other splits, two in flight, added in split order
-        float pr[2][32];
-        load_row32(e.partial + (size_t)m * e.N + nb, nvalid, pr[0]);
-        if (e.ksplit > 2) load_row32(e.partial + (size_t)e.M * e.N + (size_t)m * e.N + nb, nvalid, pr[1]);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] += pr[0][j];
-        if (e.ksplit > 2) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += pr[1][j];
-        }
-        for (int sp = 2; sp < e.ksplit - 1; ++sp) {
-          load_row32(e.partial + (size_t)sp * e.M * e.N + (size_t)m * e.N + nb, nvalid, pr[0]);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += pr[0][j];
-        }
-      }
       if (!split_out) {
         TA3N_EPI_DISPATCH(e.flags, { epilogue_row32<EPI_F>(e, m, nb, nvalid, v); })
       }
@@ -432,252 +410,6 @@ __device__ __forceinline__ void tc_epilogue(const TileCtx& ctx, const int m0, co
       }
     }
   }
-}
-
-// ---- coalesced epilogue (step kernel) -------------------------------------------------------------------
-// The epilogue above gives every lane one accumulator ROW: each of its memory instructions touches 32 different
-// 128 B lines, i.e. 32 LSU cycles per instruction, which dominates the tiles whose epilogue reads several auxiliary
-// operands (relation-discriminator data gradient).  Here a warp stages
-// its 32 x 32 accumulator chunk in shared memory ([32][36] floats, conflict-free for the 16 B accesses of both
-// passes) and re-reads it with lanes along the COLUMNS: lane = (row quarter rq, column quad cq), every global access
-// is a 16 B piece of a 128 B row segment, 4 rows per instruction.  Auxiliary operands of four rows are requested
-// together before the first is used.
-// ONE body with run-time flags (uniform branches), not one copy per flag set: the nine specialised copies of the
-// first version made the step kernel 42 k instructions (680 KB), far beyond the instruction cache.  The step planner
-// guarantees what keeps it small: N % 4 == 0, every leading dimension % 4 == 0, every pointer 16-byte aligned (no
-// scalar tails), ksplit <= 4, and no auxiliary operand on a split group (the three aux registers sets are shared
-// between {partials} and {add, gate, accumulate}).
-constexpr int TC_STAGE_LD = 36;
-constexpr int TC_EPI_STAGE_FLOATS = 32 * TC_STAGE_LD;      // per epilogue warp
-
-__device__ __forceinline__ float4 ldcg4(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
-__device__ __forceinline__ void add4(float4& a, const float4& b) {
-  a.x += b.x;
-  a.y += b.y;
-  a.z += b.z;
-  a.w += b.w;
-}
-
-// CLS selects how much of the body exists (three copies instead of one per flag set):
-//   0 = plain: alpha * accumulator (+ split-K partials)          weight gradients, partial tiles, frame dgrad
-//   1 = forward: + bias, ReLU, dropout                            every forward layer
-//   2 = everything (run-time flags)                               the data-gradient tiles with auxiliary operands
-// The per-element work of the plain class is one multiply: with run-time flag tests inside the row loops it was
-// 1300 instructions per warp and tile (5 us at 2 warps per scheduler); the lean copies are ~250.
-enum : int { EPI_CLS_PLAIN = 0, EPI_CLS_FORWARD = 1, EPI_CLS_ALL = 2 };
-__device__ __forceinline__ int epi_class(const int mode, const int flags) {
-  if (mode == TILE_PARTIAL || mode == TILE_SPLIT || flags == 0) return EPI_CLS_PLAIN;
-  if ((flags & ~(EPI_BIAS | EPI_RELU | EPI_DROP_MASK | EPI_DROP_RNG)) == 0) return EPI_CLS_FORWARD;
-  return EPI_CLS_ALL;
-}
-
-template <int kEpiWarps, int CLS>
-__device__ __forceinline__ void tc_epilogue_cls(const TileCtx& ctx, const int m0, const int n0, const int split,
-                                                const int n_iter, const int mode, const float* acc, const int ew,
-                                                const uint32_t stage) {
-  const int lane = threadIdx.x & 31;
-  const int lq = ew & 3;                // row quarter of the tile
-  const Group& e = ctx.g;               // shared memory (the task slot)
-  constexpr int kMask = CLS == EPI_CLS_PLAIN ? 0
-                        : CLS == EPI_CLS_FORWARD ? (EPI_BIAS | EPI_RELU | EPI_DROP_MASK | EPI_DROP_RNG)
-                                                 : ~0;
-  const bool split_out = mode == TILE_PARTIAL || mode == TILE_SPLIT;
-  const int f = (split_out ? 0 : e.flags) & kMask;
-  const int M = e.M, N = e.N;
-  const size_t plane = (size_t)M * N;
-  float* const obase = split_out ? e.partial + (size_t)split * plane : e.C;
-  const int ldo = split_out ? N : e.ldc;
-  constexpr int kColChunks = (TC_BN / 32) * 4 / kEpiWarps;
-  const int c0 = (ew / 4) * kColChunks;
-  const int rq = lane >> 3, cq = lane & 7;
-  // planes of raw partial sums folded in (no aux operands on split groups: the register sets are shared)
-  const int n_part = CLS == EPI_CLS_ALL ? 0 : (mode == TILE_OWNER ? e.ksplit - 1 : (mode == TILE_REDUCE ? e.ksplit : 0));
-  const float alpha = split_out ? 1.0f : (e.alpha_dev ? e.alpha * __ldg(e.alpha_dev) : e.alpha);
-  const uint64_t step = (f & EPI_DROP_RNG) ? (e.step_dev ? *e.step_dev : 0ull) : 0ull;
-  const bool drop_early = (f & (EPI_DROP_MASK | EPI_DROP_RNG)) && !(f & EPI_DROP_LATE);
-  const bool drop_late = (f & (EPI_DROP_MASK | EPI_DROP_RNG)) && (f & EPI_DROP_LATE);
-#pragma unroll 1
-  for (int c = c0; c < c0 + kColChunks; ++c) {
-    {  // accumulator chunk -> registers (lane = row) -> shared memory
-      float v[32];
-      if (n_iter > 0) {
-        acc_ld_32(acc, lq * 32 + lane, c * 32, v);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
-      }
-      __syncwarp();                     // the previous chunk's readers are done with the staging tile
-#pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        sts4(stage + (uint32_t)(lane * TC_STAGE_LD + j) * 4u, make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]));
-      __syncwarp();
-    }
-    const int n = n0 + c * 32 + cq * 4;
-    if (n >= N) continue;               // N % 4 == 0: a column quad is inside or outside as a whole
-    float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (f & EPI_BIAS) bias4 = ldcg4(e.bias + n);
-#pragma unroll 1
-    for (int half = 0; half < 2; ++half) {                 // 2 batches of 4 x (4 rows per instruction) = 32 rows
-      int rows[4];
-      bool ok[4];
-      float4 q[4], x0[4], x1[4], x2[4], x3[4];
-      float rs[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int r = (half * 4 + u) * 4 + rq;            // row of the chunk
-        rows[u] = m0 + lq * 32 + r;
-        ok[u] = rows[u] < M;
-        q[u] = lds4(stage + (uint32_t)(r * TC_STAGE_LD + cq * 4) * 4u);
-      }
-      // ---- every load of the batch first ----
-      // (every element of the auxiliary arrays is written, under a select rather than a branch: left partly
-      //  uninitialised behind `continue`s the compiler kept them in LOCAL memory and stored each load result to the
-      //  stack as it arrived -- one load in flight at a time)
-      const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const size_t m = (size_t)(ok[u] ? rows[u] : m0);        // a safe row for the masked-off lanes
-        x0[u] = x1[u] = x2[u] = zero4;
-        rs[u] = 1.0f;
-        if (n_part > 0) {
-          x0[u] = ldcg4(e.partial + m * N + n);
-          if (n_part > 1) x1[u] = ldcg4(e.partial + plane + m * N + n);
-          if (n_part > 2) x2[u] = ldcg4(e.partial + 2 * plane + m * N + n);
-          x3[u] = n_part > 3 ? ldcg4(e.partial + 3 * plane + m * N + n) : zero4;
-        } else if (CLS == EPI_CLS_ALL) {
-          if (f & EPI_ADDROW) {
-            if (e.rowscale) rs[u] = __ldcg(e.rowscale + m * e.rs_stride) + e.rs_bias;
-            x0[u] = ldcg4(e.add + m * e.ldadd + n);
-          }
-          if (f & (EPI_GATE | EPI_DPRE)) x1[u] = ldcg4(e.gate + m * e.ldgate + n);
-          if (f & EPI_ACCUM) x2[u] = ldcg4(e.C + m * e.ldc + n);
-          if (f & EPI_MULTI) {          // the gates of every dZ plane ride with the first round of loads
-            x1[u] = ldcg4(e.multi_gate[0] + m * e.ldmulti + n);           // (a MULTI group has no gate / accumulate)
-            if (e.n_multi > 1) x2[u] = ldcg4(e.multi_gate[1] + m * e.ldmulti + n);
-            x3[u] = e.n_multi > 2 ? ldcg4(e.multi_gate[2] + m * e.ldmulti + n) : zero4;
-          }
-        }
-      }
-      // ---- arithmetic + store ----
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const size_t m = (size_t)(ok[u] ? rows[u] : m0);
-        float4 v = q[u];
-        if (n_part > 0) {
-          add4(v, x0[u]);
-          if (n_part > 1) add4(v, x1[u]);
-          if (n_part > 2) add4(v, x2[u]);
-          if (n_part > 3) add4(v, x3[u]);
-        }
-        if (!split_out) {
-          float ev[4] = {v.x * alpha, v.y * alpha, v.z * alpha, v.w * alpha};
-          if (f & EPI_BIAS) {
-            ev[0] += bias4.x;
-            ev[1] += bias4.y;
-            ev[2] += bias4.z;
-            ev[3] += bias4.w;
-          }
-          if (f & EPI_RELU) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) ev[i] = fmaxf(ev[i], 0.f);
-          }
-          if (drop_early || drop_late) {
-            float df[4];
-            if (f & EPI_DROP_MASK) {
-              const uchar4 k = *reinterpret_cast<const uchar4*>(e.keep + m * e.ldkeep + n);
-              df[0] = k.x ? e.drop_scale : 0.f;
-              df[1] = k.y ? e.drop_scale : 0.f;
-              df[2] = k.z ? e.drop_scale : 0.f;
-              df[3] = k.w ? e.drop_scale : 0.f;
-            } else {
-              const uint64_t base = e.rng_offset + m * (uint64_t)N + (uint64_t)n;
-              if ((base & 3ull) == 0) {                     // the quad shares one hash (always, on the path's shapes)
-                const uint64_t hsh = rng_hash4(e.seed, step, base >> 2);
-                const uint32_t thr = rng_threshold(e.drop_p);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) df[i] = rng_keep_bits(hsh, i, thr) ? e.drop_scale : 0.f;
-              } else {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) df[i] = rng_keep(e.seed, step, base + i, e.drop_p) ? e.drop_scale : 0.f;
-              }
-            }
-            if (drop_late && (f & EPI_ADDROW)) {
-              ev[0] = fmaf(rs[u], x0[u].x, ev[0]);
-              ev[1] = fmaf(rs[u], x0[u].y, ev[1]);
-              ev[2] = fmaf(rs[u], x0[u].z, ev[2]);
-              ev[3] = fmaf(rs[u], x0[u].w, ev[3]);
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) ev[i] = df[i] != 0.f ? ev[i] * df[i] : 0.f;
-          }
-          if ((f & EPI_ADDROW) && !drop_late) {
-            ev[0] = fmaf(rs[u], x0[u].x, ev[0]);
-            ev[1] = fmaf(rs[u], x0[u].y, ev[1]);
-            ev[2] = fmaf(rs[u], x0[u].z, ev[2]);
-            ev[3] = fmaf(rs[u], x0[u].w, ev[3]);
-          }
-          if (f & EPI_GATE) {
-            ev[0] = x1[u].x > 0.f ? ev[0] : 0.f;
-            ev[1] = x1[u].y > 0.f ? ev[1] : 0.f;
-            ev[2] = x1[u].z > 0.f ? ev[2] : 0.f;
-            ev[3] = x1[u].w > 0.f ? ev[3] : 0.f;
-          }
-          if (f & EPI_ACCUM) {
-            ev[0] += x2[u].x;
-            ev[1] += x2[u].y;
-            ev[2] += x2[u].z;
-            ev[3] += x2[u].w;
-          }
-          if (f & EPI_DPRE) {
-            ev[0] = x1[u].x > 0.f ? ev[0] * e.drop_scale : 0.f;
-            ev[1] = x1[u].y > 0.f ? ev[1] * e.drop_scale : 0.f;
-            ev[2] = x1[u].z > 0.f ? ev[2] * e.drop_scale : 0.f;
-            ev[3] = x1[u].w > 0.f ? ev[3] * e.drop_scale : 0.f;
-          }
-          v = make_float4(ev[0], ev[1], ev[2], ev[3]);
-        }
-        q[u] = v;
-        if (ok[u]) *reinterpret_cast<float4*>(obase + m * ldo + n) = v;
-      }
-      if (CLS == EPI_CLS_ALL && (f & EPI_MULTI)) {      // dZ planes (gates already in x1 .. x3)
-        const int n_multi = e.n_multi;
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-          if (ok[u]) {
-            const size_t off = (size_t)rows[u] * e.ldmulti + n;
-            *reinterpret_cast<float4*>(e.multi_out[0] + off) =
-                make_float4(x1[u].x > 0.f ? q[u].x : 0.f, x1[u].y > 0.f ? q[u].y : 0.f, x1[u].z > 0.f ? q[u].z : 0.f,
-                            x1[u].w > 0.f ? q[u].w : 0.f);
-            if (n_multi > 1)
-              *reinterpret_cast<float4*>(e.multi_out[1] + off) =
-                  make_float4(x2[u].x > 0.f ? q[u].x : 0.f, x2[u].y > 0.f ? q[u].y : 0.f, x2[u].z > 0.f ? q[u].z : 0.f,
-                              x2[u].w > 0.f ? q[u].w : 0.f);
-            if (n_multi > 2)
-              *reinterpret_cast<float4*>(e.multi_out[2] + off) =
-                  make_float4(x3[u].x > 0.f ? q[u].x : 0.f, x3[u].y > 0.f ? q[u].y : 0.f, x3[u].z > 0.f ? q[u].z : 0.f,
-                              x3[u].w > 0.f ? q[u].w : 0.f);
-          }
-      }
-    }
-  }
-}
-
-// Can the step kernel's epilogue take this group?  (see tc_epilogue_coalesced)
-inline bool tc_step_group_ok(const Group& g) {
-  auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-  if (g.N % 4 != 0 || g.ldc % 4 != 0 || !a16(g.C) || g.ksplit > 4) return false;
-  if (g.ksplit > 1 && (g.flags & (EPI_ADDROW | EPI_GATE | EPI_ACCUM | EPI_DPRE | EPI_MULTI))) return false;
-  if ((g.flags & EPI_BIAS) && !a16(g.bias)) return false;
-  if ((g.flags & EPI_DROP_MASK) && (g.ldkeep % 4 != 0 || (reinterpret_cast<uintptr_t>(g.keep) & 3u) != 0)) return false;
-  if ((g.flags & EPI_ADDROW) && (g.ldadd % 4 != 0 || !a16(g.add))) return false;
-  if ((g.flags & (EPI_GATE | EPI_DPRE)) && (g.ldgate % 4 != 0 || !a16(g.gate))) return false;
-  if (g.flags & EPI_MULTI) {
-    if (g.ldmulti % 4 != 0 || g.n_multi < 1 || g.n_multi > 3) return false;
-    if (g.flags & (EPI_GATE | EPI_DPRE | EPI_ACCUM)) return false;      // their registers carry the plane gates
-    for (int p = 0; p < g.n_multi; ++p)
-      if (!a16(g.multi_gate[p]) || !a16(g.multi_out[p])) return false;
-  }
-  return true;
 }
 
 // chunk range [c_begin, c_begin + n_iter) of split `split` of the group staged in ctx
@@ -734,7 +466,7 @@ seg_gemm_tc_kernel(const __grid_constant__ GemmTable tab, const __grid_constant_
       tc_produce<TC_STAGES>(ctx, maps.m, A_KMAJ, B_KMAJ, tab.pad_, m0, n0, c_begin, n_iter, smem, &sh, 0u);
   } else {
     float d[64];
-    tc_consume<TC_STAGES>(A_KMAJ, B_KMAJ, n_iter, smem, &sh, 0u, d);
+    tc_consume<TC_STAGES>(A_KMAJ, B_KMAJ, n_iter, smem, &sh, d);
     consumer_sync();                    // every MMA has read the ring: it becomes the accumulator tile
     float* acc = reinterpret_cast<float*>(smem);
     tc_store_acc(acc, d, threadIdx.x);
@@ -1163,7 +895,6 @@ inline PFN_encodeTiled encode_fn() {
 struct DeviceInfo {
   int sm_count = 0;
   bool configured[4] = {false, false, false, false};        // seg_gemm_tc_kernel, per operand layout
-  bool step_configured = false;      // step_kernel.cuh kernels (ta3n_api.cu)
   bool x3_configured[4] = {false, false, false, false};      // seg_gemm_tc_x3_kernel, per operand layout
 };
 inline std::mutex& device_mu() {

@@ -146,8 +146,7 @@ __device__ __forceinline__ float apply_epilogue(const Group& g, int m, int n, fl
 }
 
 // 32 consecutive floats p[0..31] of one row -> registers; 16 B vector loads when possible.  ld.global.cg: read at L2
-// (no reuse in L1 anyway), so that inside the persistent step kernel data written by another SM earlier in the SAME
-// launch is never served from a stale L1 line.
+// (no reuse in L1 anyway).
 __device__ __forceinline__ void load_row32(const float* p, int nvalid, float (&r)[32]) {
   if (nvalid >= 32 && (reinterpret_cast<uintptr_t>(p) & 15u) == 0) {
 #pragma unroll

@@ -1,14 +1,13 @@
-// step_plan.cuh -- host side of the fused training step: turns a ta3n_step_desc into
-//   (a) a StepProgram: the grouped GEMMs of every dependency level (the same GemmPlan tables the per-op API uses),
-//       the arguments of the fused per-video row task and the column-sum jobs;
-//   (b) either a sequence of launches (phased executor) or the task graph of the persistent step kernel.
+// step_plan.cuh -- host side of the training step: turns a ta3n_step_desc into a StepProgram: the grouped GEMMs of
+// every dependency level (the same GemmPlan tables the per-op API uses), the arguments of the fused per-video row
+// task and the column-sum jobs.  ta3n_step_run_phased launches it level by level.
 #pragma once
 
 #include <algorithm>
-#include <map>
 #include <vector>
 
-#include "step_kernel.cuh"
+#include "gemm_wgmma.cuh"
+#include "step_rows.cuh"
 
 namespace ta3n {
 
@@ -50,32 +49,15 @@ struct StepScratch {
   float *g_video, *g_dom, *g_frame, *g_rel, *Pt, *dHv, *Gc, *G, *dHid, *dHf, *d_feat, *d_feat_rel, *dz, *row_loss, *frame_loss;
 };
 
-// stages whose completion a weight-gradient group / column-sum job waits for
-enum : int { DEP_FRAME = 1, DEP_HEADS = 2, DEP_RELBWD = 4, DEP_DZ = 8, DEP_DFEAT = 16 };
-struct StepJob {        // a column-sum job and the stages whose outputs it reads (DEP_* mask, at most two bits)
-  WColsumJob job;
-  int dep;
-};
-
 struct StepProgram {
   StepRelLayout L;
   int M, MT, Rs, Rt;
   StepScratch sc;
   GemmPlan g1, g2, g3, g4a, g4b, g5, g6, g7;
-  int g2_frame_group;                 // index of the frame-discriminator hidden group inside g2 (TRN groups follow)
-  int g5_frame_group;                 // index of the frame dgrad group inside g5 (relation groups come first)
-  std::vector<int> g7_dep;            // per group of g7: DEP_* mask of the stages that complete its operands
   TailArgs tail;
-  std::vector<StepJob> jobs;
+  std::vector<WColsumJob> jobs;
   size_t scratch_bytes;               // bytes of the fixed scratch tensors at the start of the workspace
 };
-
-inline size_t step_fixed_scratch_floats(int M, int T, int F, int H, int C, int R, int n_rel) {
-  auto r = [](size_t n) { return (n + 63) & ~size_t(63); };
-  const size_t MT = (size_t)M * T;
-  return r((size_t)M * C) + r((size_t)M * 2) + r(MT * 2) + 2 * r((size_t)M * R * 2) + 3 * r((size_t)M * H) +
-         r((size_t)R * M * H) + r(MT * F) + r(MT * F) + r((size_t)M * R * H) + r((size_t)n_rel * M * H) + r((size_t)M) + r(MT);
-}
 
 // dry: only sizes are wanted (workspace query) -- scratch pointers are placeholders that are never dereferenced
 inline int build_step_program(const ta3n_step_desc* d, StepProgram* P, bool dry = false) {
@@ -84,9 +66,9 @@ inline int build_step_program(const ta3n_step_desc* d, StepProgram* P, bool dry 
   const StepRelLayout& L = P->L;
   const int T = d->T, D = d->D, F = d->F, H = d->H, C = d->C, R = L.R;
   TA3N_REQUIRE(d->Bs >= 1 && d->Bt >= 0 && T == L.T && D > 0 && F > 0 && H > 0 && C >= 1, "bad sizes");
-  TA3N_REQUIRE((H == 128 || H == 256) && F % 4 == 0 && D % 4 == 0, "fused step needs H in {128, 256}, F % 4 == 0, D % 4 == 0");
-  TA3N_REQUIRE(L.R <= 32, "fused step: at most 32 relation scales");
-  TA3N_REQUIRE(T <= kTailMaxT && C <= kTailMaxC, "fused step: T <= 32, C <= 128");
+  TA3N_REQUIRE((H == 128 || H == 256) && F % 4 == 0 && D % 4 == 0, "step program needs H in {128, 256}, F % 4 == 0, D % 4 == 0");
+  TA3N_REQUIRE(L.R <= 32, "step program: at most 32 relation scales");
+  TA3N_REQUIRE(T <= kTailMaxT && C <= kTailMaxC, "step program: T <= 32, C <= 128");
   TA3N_REQUIRE(d->x_src && (d->Bt == 0 || d->x_tgt) && d->labels && d->beta_dev && d->loss, "null input");
   TA3N_REQUIRE(d->W_sh && d->b_sh && d->W1f && d->b1f && d->W2f && d->b2f && d->Wc && d->bc && d->W1v && d->b1v &&
                    d->W2v && d->b2v && d->W_trn_host && d->b_trn_host && d->W1r_host && d->b1r_host && d->W2r_host &&
@@ -121,7 +103,7 @@ inline int build_step_program(const ta3n_step_desc* d, StepProgram* P, bool dry 
   sc.dz = take((size_t)L.n_rel * M * H);
   sc.row_loss = take((size_t)M);
   sc.frame_loss = take((size_t)MT);
-  if (!sc.frame_loss) return fail(TA3N_ERR_WORKSPACE, "fused step: workspace too small (%zu bytes)", d->workspace_bytes);
+  if (!sc.frame_loss) return fail(TA3N_ERR_WORKSPACE, "step program: workspace too small (%zu bytes)", d->workspace_bytes);
   P->scratch_bytes = arena.used;
 
   const DropArgs di = make_drop(&d->drop_i), dv = make_drop(&d->drop_v);
@@ -167,7 +149,6 @@ inline int build_step_program(const ta3n_step_desc* d, StepProgram* P, bool dry 
     p = GemmPlan();
     p.label = "step_fwd_batch";
     p.precise = true;
-    P->g2_frame_group = 0;
     Group& gf = p.add_group(MT, F, d->hid_f, F);
     gf.flags = EPI_BIAS | EPI_RELU;
     gf.bias = d->b1f;
@@ -333,7 +314,6 @@ inline int build_step_program(const ta3n_step_desc* d, StepProgram* P, bool dry 
       }
       p.add_seg(sc.dHid + (size_t)i * plane, H, d->W1r_host[i], H, H);
     }
-    P->g5_frame_group = R;
     Group& gf = p.add_group(MT, F, sc.d_feat, F);
     gf.alpha = -1.0f;
     gf.alpha_dev = d->beta_dev + 2;
@@ -370,14 +350,11 @@ inline int build_step_program(const ta3n_step_desc* d, StepProgram* P, bool dry 
     p.label = "step_wgrad";
     p.a_kmaj = false;
     p.b_kmaj = false;
-    P->g7_dep.clear();
     p.add_group(F, D, d->dW_sh, D);                                     // shared layer: d_pre^T x
     if (Rs > 0) p.add_seg(sc.d_feat, F, d->x_src, D, Rs);
     if (Rt > 0) p.add_seg(sc.d_feat + (size_t)Rs * F, F, d->x_tgt, D, Rt);
-    P->g7_dep.push_back(DEP_DFEAT);
     p.add_group(F, F, d->dW1f, F);                                      // frame discriminator layer 1
     p.add_seg(sc.dHf, F, d->feat, F, MT);
-    P->g7_dep.push_back(DEP_FRAME);
     for (int i = 0; i < R; ++i) {                                       // TRN: dW_i[:, jF:(j+1)F] = sum_r dZ^T x[tau[j]]
       const int s = L.scale_size[i];
       TA3N_REQUIRE(d->dW_trn_host[i] && d->db_trn_host[i], "null TRN gradient");
@@ -385,82 +362,59 @@ inline int build_step_program(const ta3n_step_desc* d, StepProgram* P, bool dry 
         p.add_group(H, F, d->dW_trn_host[i] + (size_t)j * F, s * F);
         for (int q = L.rel_begin[i]; q < L.rel_begin[i + 1]; ++q)
           p.add_seg(sc.dz + (size_t)q * plane, H, d->feat + (size_t)L.frames[L.slot_begin[q] + j] * F, ldx, M);
-        P->g7_dep.push_back(DEP_DZ);
       }
     }
     for (int i = 0; i < R; ++i) {                                       // relation discriminators layer 1
       TA3N_REQUIRE(d->dW1r_host[i] && d->db1r_host[i] && d->dW2r_host[i] && d->db2r_host[i], "null relation gradient");
       p.add_group(H, H, d->dW1r_host[i], H);
       p.add_seg(sc.dHid + (size_t)i * plane, H, d->feat_rel + (size_t)i * H, R * H, M);
-      P->g7_dep.push_back(DEP_RELBWD);
     }
     p.add_group(H, H, d->dW1v, H);                                      // video discriminator layer 1
     p.add_seg(sc.dHv, H, d->dropped, H, M);
-    P->g7_dep.push_back(DEP_HEADS);
     // (the classifier's weight gradient dWc [C, H] is a skinny reduction over the videos: a weighted column sum below)
   }
   // ---- column sums: bias gradients, skinny head weight gradients, the scalar loss ----
   {
-    P->jobs.clear();
     ColsumPlan cs;
-    auto push = [&](int dep) {
-      StepJob j;
-      j.job = cs.jobs.back();
-      j.dep = dep;
-      P->jobs.push_back(j);
-    };
     cs.add(d->db_sh, F, F);
     cs.seg(sc.d_feat, MT);
-    push(DEP_DFEAT);
     cs.add(d->db1f, F, F);
     cs.seg(sc.dHf, MT);
-    push(DEP_FRAME);
     cs.add_weighted(d->dW2f, F, 2, F, F, 2);
     cs.seg(d->hid_f, MT, sc.g_frame);
-    push(DEP_FRAME);
     cs.add(d->db2f, 2, 2);
     cs.seg(sc.g_frame, MT);
-    push(DEP_FRAME);
     for (int i = 0; i < R; ++i) {
       cs.add(d->db_trn_host[i], H, H);
       for (int q = L.rel_begin[i]; q < L.rel_begin[i + 1]; ++q) cs.seg(sc.dz + (size_t)q * plane, M);
-      push(DEP_DZ);
     }
     for (int i = 0; i < R; ++i) {
       cs.add_weighted(d->dW2r_host[i], H, 2, H, H, R * 2);
       cs.seg(d->hid_r + (size_t)i * plane, M, sc.Pt + (size_t)i * 2);
-      push(DEP_RELBWD);
       cs.add(d->db2r_host[i], 2, R * 2);
       cs.seg(sc.Pt + (size_t)i * 2, M);
-      push(DEP_RELBWD);
       cs.add(d->db1r_host[i], H, H);
       cs.seg(sc.dHid + (size_t)i * plane, M);
-      push(DEP_RELBWD);
     }
     cs.add_weighted(d->dWc, H, C, H, H, C);
     cs.seg(d->dropped, M, sc.g_video);
-    push(DEP_HEADS);
     cs.add(d->dbc, C, C);
     cs.seg(sc.g_video, M);
-    push(DEP_HEADS);
     cs.add_weighted(d->dW2v, H, 2, H, H, 2);
     cs.seg(d->hid_v, M, sc.g_dom);
-    push(DEP_HEADS);
     cs.add(d->db2v, 2, 2);
     cs.seg(sc.g_dom, M);
-    push(DEP_HEADS);
     cs.add(d->db1v, H, H);
     cs.seg(sc.dHv, M);
-    push(DEP_HEADS);
     cs.add(d->loss, 1, 1);                 // the scalar loss: video / relation level terms + frame level terms
     cs.seg(sc.row_loss, M);
     cs.seg(sc.frame_loss, MT);
-    push(DEP_HEADS | DEP_FRAME);
+    P->jobs = cs.jobs;
   }
   return TA3N_OK;
 }
 
-// row splits / vector flag of a column-sum job (shared by both executors so that they sum in the same order)
+// row splits / vector flag of a column-sum job
 inline void step_prepare_job(WColsumJob* j) {
   int rows_total = 0;
   bool vec = (j->N % 4 == 0) && (j->ld % 4 == 0);
@@ -476,536 +430,24 @@ inline void step_prepare_job(WColsumJob* j) {
   (void)rows_total;
 }
 
-inline bool step_split_enabled() {      // TA3N_STEP_NOSPLIT=1: no split-K in the task graph (bit-compare with the phased executor)
-  static const bool on = []() {
-    const char* e = getenv("TA3N_STEP_NOSPLIT");
-    return !(e && e[0] == '1');
-  }();
-  return on;
-}
-
-// ---- split factors of the step kernel's GEMM groups ----
-inline int step_slabs(const GemmPlan& p, const Group& g) {
-  int n = 0;
-  for (int k = 0; k < g.seg_count; ++k) n += (p.segs[g.seg_begin + k].len + TC_BK - 1) / TC_BK;
-  return n;
-}
-inline int step_tiles(const Group& g) { return ((g.M + TC_BM - 1) / TC_BM) * ((g.N + TC_BN - 1) / TC_BN); }
-
-// forward-critical launch with too few tiles for the machine: ~1.6 tasks per SM, >= 8 slabs per task
-inline int step_split_critical(int tiles, int slabs, int sm_count) {
-  if (!step_split_enabled()) return 1;
-  int ks = (int)((1.6 * sm_count) / std::max(tiles, 1) + 0.5);
-  ks = std::max(1, std::min(ks, 4));
-  while (ks > 1 && slabs / ks < 8) --ks;
-  return ks;
-}
-// weight-gradient tiles are fillers: keep a task below ~24 slabs so that it cannot block a critical stage for long
-inline int step_split_filler(int slabs) {
-  if (!step_split_enabled()) return 1;
-  int ks = std::max(1, std::min(4, (slabs + 23) / 24));
-  while (ks > 1 && slabs / ks < 8) --ks;
-  return ks;
-}
-
-struct BuiltPlan {
-  std::vector<StepTask> tasks;    // queue 0's tasks, then queue 1's, ...
-  int queue_begin[kStepQueues + 1];
-  std::vector<StepGroup> groups;
-  std::vector<SegLite> segs;
-  std::vector<CUtensorMap> maps;
-  std::vector<WColsumJob> jobs;
-  int n_counters = 0;
-  int n_gemm_tiles = 0;
-  size_t partial_floats = 0;      // split-K partials + column-sum partials (carved after the fixed scratch)
-};
-
-struct StepHandle {              // what ta3n_step_run needs on the host (TA3N_STEP_HANDLE_BYTES)
-  StepHeader hd;
-  int magic;
-  int n_gemm_tiles;
-  int smem_bytes;
-  int grid;
-};
-static_assert(sizeof(StepHandle) <= TA3N_STEP_HANDLE_BYTES, "handle too large");
-
-// Build the task graph.  `partial_base` = device memory for split-K / column-sum partials (may be null when only
-// counting), carved in a fixed order.
-inline int build_task_graph(const StepProgram& P, int sm_count, float* partial_base, size_t partial_cap_floats,
-                            BuiltPlan* B) {
-  const StepRelLayout& L = P.L;
-  const int T = L.T, R = L.R, M = P.M, MT = P.MT;
-  size_t pused = 0;
-  auto carve = [&](size_t n) -> float* {
-    n = (n + 63) & ~size_t(63);
-    float* p = partial_base ? partial_base + pused : nullptr;
-    pused += n;
-    return p;
-  };
-  int nc = 0;
-  auto counters = [&](int n) {
-    const int b = nc;
-    nc += n;
-    return b;
-  };
-  std::map<MapKey, int> map_index;
-  auto map_of = [&](const MapKey& k) -> int {
-    auto it = map_index.find(k);
-    if (it != map_index.end()) return it->second;
-    const int idx = (int)B->maps.size();
-    CUtensorMap m;
-    memset(&m, 0, sizeof(m));
-    if (partial_base != nullptr && encode_map(k, &m) != TA3N_OK) return -1;
-    B->maps.push_back(m);
-    map_index[k] = idx;
-    return idx;
-  };
-  // register a plan's groups; returns the index of its first StepGroup
-  auto add_groups = [&](const GemmPlan& p, const std::vector<int>& ksplit) -> int {
-    const int first = (int)B->groups.size();
-    for (size_t gi = 0; gi < p.groups.size(); ++gi) {
-      StepGroup sg;
-      memset(&sg, 0, sizeof(sg));
-      sg.g = p.groups[gi];
-      sg.a_kmaj = p.a_kmaj ? 1 : 0;
-      sg.b_kmaj = p.b_kmaj ? 1 : 0;
-      const bool a3d = !p.a_kmaj && sg.g.M % 32 == 0, b3d = !p.b_kmaj && sg.g.N % 32 == 0;
-      sg.pad_flags = (a3d ? 1 : 0) | (b3d ? 2 : 0);
-      sg.seg_begin = (int)B->segs.size();
-      sg.g.tiles_m = (sg.g.M + TC_BM - 1) / TC_BM;
-      sg.g.tiles_n = (sg.g.N + TC_BN - 1) / TC_BN;
-      sg.g.ksplit = ksplit[gi];
-      sg.g.fix_slot = -1;
-      sg.g.partial = sg.g.ksplit > 1 ? carve((size_t)sg.g.ksplit * sg.g.M * sg.g.N) : nullptr;
-      if (!tc_step_group_ok(sg.g)) {
-        fail(TA3N_ERR_UNSUPPORTED, "fused step: a group of %s breaks the epilogue's alignment rules (N %d, ldc %d, flags %d)",
-             p.label, sg.g.N, sg.g.ldc, sg.g.flags);
-        return -1;
-      }
-      for (int k = 0; k < sg.g.seg_count; ++k) {
-        const Seg& s = p.segs[p.groups[gi].seg_begin + k];
-        if (!tc_operand_ok(s.A, s.lda) || !tc_operand_ok(s.B, s.ldb) || s.len <= 0) {
-          fail(TA3N_ERR_UNSUPPORTED, "fused step: operand of %s is not 16-byte aligned / strided (lda %d ldb %d)", p.label,
-               s.lda, s.ldb);
-          return -1;
-        }
-        MapKey ka, kb;
-        tc_seg_keys(s, sg.g, p.a_kmaj, p.b_kmaj, a3d, b3d, &ka, &kb);
-        SegLite l;
-        l.A = s.A;
-        l.B = s.B;
-        l.len = s.len;
-        l.lda = s.lda;
-        l.ldb = s.ldb;
-        const int ia = map_of(ka), ib = map_of(kb);
-        if (ia < 0 || ib < 0) return -1;
-        l.amap = (unsigned short)ia;
-        l.bmap = (unsigned short)ib;
-        B->segs.push_back(l);
-      }
-      sg.g.seg_begin = 0;      // the kernel stages the group's segments at ctx.seg[0..]
-      B->groups.push_back(sg);
+// The column-sum launches of the step: the jobs in program order, at most kMaxWColsumJobs per launch, the row-split
+// partials of every job carved from `arena` in that order.  launch(table, last) is called once per launch.  Both the
+// run and the workspace query walk the jobs through here, so the size and the carve cannot drift apart.
+template <class Launch>
+inline int step_colsum_batches(const StepProgram& P, Arena* arena, Launch&& launch) {
+  size_t i = 0;
+  while (i < P.jobs.size()) {
+    WColsumTable tab;
+    tab.n_jobs = 0;
+    while (i < P.jobs.size() && tab.n_jobs < kMaxWColsumJobs) {
+      WColsumJob j = P.jobs[i++];
+      step_prepare_job(&j);
+      j.partial = arena->floats((size_t)j.nsplit * j.N2 * j.N);
+      if (!j.partial) return fail(TA3N_ERR_WORKSPACE, "step program: column-sum workspace too small");
+      tab.job[tab.n_jobs++] = j;
     }
-    return first;
-  };
-  struct Dep {
-    int b = 0, e = 0, v = 0;
-  };
-  // Emit the tile tasks of one group.  sig(mb) = counter bumped by the final tile of row block mb (or -1).
-  auto emit_group = [&](std::vector<StepTask>* out, int gidx, const Dep& d0, const std::function<Dep(int m0)>& dep_of_rows,
-                        const std::function<int(int mb)>& sig, int sig_total = -1) {
-    const Group& g = B->groups[gidx].g;
-    const int pc = g.ksplit > 1 ? counters(g.tiles_m * g.tiles_n) : -1;
-    for (int tm = 0; tm < g.tiles_m; ++tm)
-      for (int tn = 0; tn < g.tiles_n; ++tn)
-        for (int sp = 0; sp < g.ksplit; ++sp) {
-          StepTask t;
-          memset(&t, 0, sizeof(t));
-          t.type = TASK_GEMM;
-          t.group = gidx;
-          t.m0 = tm * TC_BM;
-          t.n0 = tn * TC_BN;
-          t.split = sp;
-          // split-K: every split writes its raw partial; the last one to arrive at the tile's counter reduces them
-          // in split order and announces the tile (TILE_SPLIT, step_kernel.cuh) -- no split waits for another
-          t.mode = g.ksplit == 1 ? TILE_FINAL : TILE_SPLIT;
-          t.split_counter = g.ksplit > 1 ? pc + tm * g.tiles_n + tn : -1;
-          Dep dr = dep_of_rows ? dep_of_rows(t.m0) : d0;
-          t.wait_begin[0] = dr.b;
-          t.wait_end[0] = dr.e;
-          t.wait_val[0] = dr.v;
-          if (dep_of_rows && d0.e > d0.b) {       // second static range
-            t.wait_begin[1] = d0.b;
-            t.wait_end[1] = d0.e;
-            t.wait_val[1] = d0.v;
-          }
-          t.signal = sig ? sig(tm) : -1;
-          t.signal2 = sig_total;
-          out->push_back(t);
-          ++B->n_gemm_tiles;
-        }
-    return 0;
-  };
-  auto sort_by_slabs = [&](std::vector<StepTask>* v) {
-    std::stable_sort(v->begin(), v->end(), [&](const StepTask& a, const StepTask& b) {
-      const Group& ga = B->groups[a.group].g;
-      const Group& gb = B->groups[b.group].g;
-      int sa = 0, sb = 0;
-      for (int k = 0; k < ga.seg_count; ++k) sa += (B->segs[B->groups[a.group].seg_begin + k].len + TC_BK - 1) / TC_BK;
-      for (int k = 0; k < gb.seg_count; ++k) sb += (B->segs[B->groups[b.group].seg_begin + k].len + TC_BK - 1) / TC_BK;
-      sa = (sa + ga.ksplit - 1) / ga.ksplit;
-      sb = (sb + gb.ksplit - 1) / gb.ksplit;
-      return sa > sb;
-    });
-  };
-  // the queues: 0 = spine, 1 .. kStepQueues-2 = row-block chains, kStepQueues-1 = fillers
-  std::vector<StepTask> queue[kStepQueues];
-  constexpr int kFill = kStepQueues - 1;
-  auto chain_q = [&](int mb) { return 1 + mb % (kStepQueues - 2); };
-  auto append = [&](int q, const std::vector<StepTask>& v) { queue[q].insert(queue[q].end(), v.begin(), v.end()); };
-  const int nmb = (M + TC_BM - 1) / TC_BM;              // row blocks of a [videos] operand
-  const int nfb = (MT + TC_BM - 1) / TC_BM;             // row blocks of a [frames] operand
-  auto one = [](int c, int v) {
-    Dep d;
-    d.b = c;
-    d.e = c + 1;
-    d.v = v;
-    return d;
-  };
-
-  // ================= S1: shared layer (spine) =================
-  std::vector<int> ks1;
-  for (const Group& g : P.g1.groups) ks1.push_back(step_split_critical(step_tiles(P.g1.groups[0]) + (P.g1.groups.size() > 1 ? step_tiles(P.g1.groups[1]) : 0), step_slabs(P.g1, g), sm_count));
-  const int g1 = add_groups(P.g1, ks1);
-  if (g1 < 0) return TA3N_ERR_UNSUPPORTED;
-  // row space of `feat`: blocks of the source group, then of the target group
-  struct RowBlock {
-    int r0, r1, c;
-  };
-  std::vector<RowBlock> feat_blocks;
-  std::vector<int> g1_cbase;
-  {
-    int row0 = 0;
-    for (size_t gi = 0; gi < P.g1.groups.size(); ++gi) {
-      const Group& g = P.g1.groups[gi];
-      const int nb = (g.M + TC_BM - 1) / TC_BM;
-      const int cb = counters(nb);
-      g1_cbase.push_back(cb);
-      for (int b = 0; b < nb; ++b) feat_blocks.push_back({row0 + b * TC_BM, row0 + std::min((b + 1) * TC_BM, g.M), cb + b});
-      row0 += g.M;
-    }
+    TA3N_TRY(launch(tab, i >= P.jobs.size()));
   }
-  const int need1 = (P.g1.groups[0].N + TC_BN - 1) / TC_BN;
-  auto feat_rows = [&](int r0, int r1) {                // counters of the S1 blocks that produce feat rows [r0, r1)
-    Dep d;
-    d.b = 1 << 30;
-    d.e = -1;
-    d.v = need1;
-    for (const RowBlock& rb : feat_blocks)
-      if (rb.r0 < r1 && rb.r1 > r0) {
-        d.b = std::min(d.b, rb.c);
-        d.e = std::max(d.e, rb.c + 1);
-      }
-    if (d.e < 0) d.b = d.e = 0;
-    return d;
-  };
-  for (size_t gi = 0; gi < P.g1.groups.size(); ++gi) {
-    std::vector<StepTask> v;
-    const int cb = g1_cbase[gi];
-    if (emit_group(&v, g1 + (int)gi, Dep(), nullptr, [cb](int mb) { return cb + mb; }) != 0) return TA3N_ERR_INVALID;
-    append(0, v);       // row block after row block: the consumers of the first rows start while the last are computed
-  }
-  // ================= S2: TRN relations (spine) + frame-discriminator hidden layer (filler) =================
-  // the longest relation tiles (scale 0: 80 K slabs at cfg2) set this stage's critical path: split them
-  std::vector<int> ones2(P.g2.groups.size(), 1);
-  if (step_split_enabled())
-    for (size_t gi = 1; gi < P.g2.groups.size(); ++gi) ones2[gi] = std::min(4, std::max(1, (step_slabs(P.g2, P.g2.groups[gi]) + 39) / 40));
-  const int g2 = add_groups(P.g2, ones2);
-  if (g2 < 0) return TA3N_ERR_UNSUPPORTED;
-  const int c2f = counters(nfb);                        // hid_f row blocks
-  const int need2f = (P.g2.groups[0].N + TC_BN - 1) / TC_BN;
-  const int c2t = counters(nmb * L.n_rel);              // act: [row block][relation]
-  const int need2t = (P.g2.groups[1].N + TC_BN - 1) / TC_BN;
-  {
-    std::vector<StepTask> v;
-    for (int q = 0; q < L.n_rel; ++q)
-      if (emit_group(&v, g2 + 1 + q, Dep(), [&](int m0) { return feat_rows(T * m0, T * std::min(m0 + TC_BM, M)); },
-                     [=](int mb) { return c2t + mb * L.n_rel + q; }) != 0)
-        return TA3N_ERR_INVALID;
-    sort_by_slabs(&v);
-    std::stable_sort(v.begin(), v.end(), [](const StepTask& a, const StepTask& b) { return a.m0 < b.m0; });   // block-major
-    append(0, v);
-    std::vector<StepTask> vf;
-    if (emit_group(&vf, g2 + 0, Dep(), [&](int m0) { return feat_rows(m0, std::min(m0 + TC_BM, MT)); },
-                   [=](int mb) { return c2f + mb; }) != 0)
-      return TA3N_ERR_INVALID;
-    append(kFill, vf);
-  }
-  // ================= frame branch (filler): frame rows -> frame dgrad =================
-  // frame row tasks never straddle a 128-row block
-  const int c4f = counters(nfb);
-  const int c4f_total = counters(1);
-  std::vector<int> frame_tasks_of(nfb, 0);
-  int n_frame_tasks = 0;
-  for (int fb = 0; fb < nfb; ++fb)
-    for (int r0 = fb * TC_BM; r0 < std::min((fb + 1) * TC_BM, MT); r0 += kRowFrames) {
-      StepTask t;
-      memset(&t, 0, sizeof(t));
-      t.type = TASK_FRAME;
-      t.m0 = r0;
-      t.n0 = std::min(kRowFrames, std::min((fb + 1) * TC_BM, MT) - r0);
-      t.wait_begin[0] = c2f + fb;
-      t.wait_end[0] = c2f + fb + 1;
-      t.wait_val[0] = need2f;
-      t.signal = c4f + fb;
-      t.signal2 = c4f_total;
-      queue[kFill].push_back(t);
-      frame_tasks_of[fb]++;
-      n_frame_tasks++;
-    }
-  // ================= S3 .. S5: the video-level chains, one per row block =================
-  std::vector<int> ones3(P.g3.groups.size(), 1);
-  const int g3 = add_groups(P.g3, ones3);
-  if (g3 < 0) return TA3N_ERR_UNSUPPORTED;
-  const int g4a = add_groups(P.g4a, std::vector<int>(1, 1));
-  const int g4b = add_groups(P.g4b, std::vector<int>(1, 1));
-  std::vector<int> ones5(P.g5.groups.size(), 1);
-  const int g5 = add_groups(P.g5, ones5);
-  if (g4a < 0 || g4b < 0 || g5 < 0) return TA3N_ERR_UNSUPPORTED;
-  const int c3 = counters(nmb * R);                     // hid_r: [row block][scale]
-  const int need3 = (P.g3.groups[0].N + TC_BN - 1) / TC_BN;
-  const int c4a = counters(nmb);                        // relpool tasks of a row block
-  const int c4b = counters(nmb);                        // hid_v tiles
-  const int c4c = counters(nmb);                        // heads tasks
-  const int c4c_total = counters(1);
-  const int c4d = counters(nmb);                        // G tiles
-  const int c4e = counters(nmb);                        // relbwd tasks
-  const int c4e_total = counters(1);
-  const int c5r = counters(nmb * R);
-  const int c5r_total = counters(1);
-  const int need5r = (P.g5.groups[0].N + TC_BN - 1) / TC_BN;
-  const int c5f = counters(nfb);
-  const int need5f = (P.g5.groups[P.g5_frame_group].N + TC_BN - 1) / TC_BN;
-  const int need4 = (P.g4a.groups[0].N + TC_BN - 1) / TC_BN;
-  std::vector<int> row_tasks_of(nmb, 0);
-  int n_row_tasks = 0;
-  for (int mb = 0; mb < nmb; ++mb) {
-    row_tasks_of[mb] = (std::min((mb + 1) * TC_BM, M) - mb * TC_BM + kRowVideos - 1) / kRowVideos;
-    n_row_tasks += row_tasks_of[mb];
-  }
-  auto emit_rows = [&](int kind, int mb, const Dep& d, int sig, int sig_total) {
-    for (int v0 = mb * TC_BM; v0 < std::min((mb + 1) * TC_BM, M); v0 += kRowVideos) {
-      StepTask t;
-      memset(&t, 0, sizeof(t));
-      t.type = TASK_ROW;
-      t.mode = kind;
-      t.m0 = v0;
-      t.n0 = std::min(kRowVideos, std::min((mb + 1) * TC_BM, M) - v0);
-      t.wait_begin[0] = d.b;
-      t.wait_end[0] = d.e;
-      t.wait_val[0] = d.v;
-      t.signal = sig;
-      t.signal2 = sig_total;
-      queue[chain_q(mb)].push_back(t);
-    }
-  };
-  // tiles of one row block of a group (emit_group emits all blocks: filter)
-  auto block_tiles = [&](const std::vector<StepTask>& v, int mb) {
-    std::vector<StepTask> o;
-    for (const StepTask& t : v)
-      if (t.m0 / TC_BM == mb) o.push_back(t);
-    return o;
-  };
-  {
-    std::vector<StepTask> v3, v4a, v4b, v5;
-    for (int i = 0; i < R; ++i)
-      if (emit_group(&v3, g3 + i, Dep(),
-                     [&, i](int m0) {
-                       Dep d;
-                       d.b = c2t + (m0 / TC_BM) * L.n_rel + L.rel_begin[i];
-                       d.e = c2t + (m0 / TC_BM) * L.n_rel + L.rel_begin[i + 1];
-                       d.v = need2t;
-                       return d;
-                     },
-                     [=](int mb) { return c3 + mb * R + i; }) != 0)
-        return TA3N_ERR_INVALID;
-    sort_by_slabs(&v3);
-    if (emit_group(&v4a, g4a, Dep(), [&](int m0) { return one(c4a + m0 / TC_BM, row_tasks_of[m0 / TC_BM]); },
-                   [=](int mb) { return c4b + mb; }) != 0)
-      return TA3N_ERR_INVALID;
-    if (emit_group(&v4b, g4b, Dep(), [&](int m0) { return one(c4c + m0 / TC_BM, row_tasks_of[m0 / TC_BM]); },
-                   [=](int mb) { return c4d + mb; }) != 0)
-      return TA3N_ERR_INVALID;
-    for (int i = 0; i < R; ++i)
-      if (emit_group(&v5, g5 + i, Dep(), [&](int m0) { return one(c4e + m0 / TC_BM, row_tasks_of[m0 / TC_BM]); },
-                     [=](int mb) { return c5r + mb * R + i; }, c5r_total) != 0)
-        return TA3N_ERR_INVALID;
-    for (int mb = 0; mb < nmb; ++mb) {
-      const int q = chain_q(mb);
-      append(q, block_tiles(v3, mb));
-      Dep d3;
-      d3.b = c3 + mb * R;
-      d3.e = c3 + (mb + 1) * R;
-      d3.v = need3;
-      emit_rows(ROW_RELPOOL, mb, d3, c4a + mb, -1);
-      append(q, block_tiles(v4a, mb));
-      emit_rows(ROW_HEADS, mb, one(c4b + mb, need4), c4c + mb, c4c_total);
-      append(q, block_tiles(v4b, mb));
-      emit_rows(ROW_RELBWD, mb, one(c4d + mb, need4), c4e + mb, c4e_total);
-      append(q, block_tiles(v5, mb));
-    }
-    // frame dgrad (filler): its A operand dHf comes from the frame row tasks of the same 128-row block
-    std::vector<StepTask> vf;
-    if (emit_group(&vf, g5 + P.g5_frame_group, Dep(), [&](int m0) { return one(c4f + m0 / TC_BM, frame_tasks_of[m0 / TC_BM]); },
-                   [=](int mb) { return c5f + mb; }) != 0)
-      return TA3N_ERR_INVALID;
-    append(kFill, vf);
-  }
-  // ================= weight gradients and column sums =================
-  std::vector<int> ks7;
-  for (size_t gi = 0; gi < P.g7.groups.size(); ++gi) ks7.push_back(step_split_filler(step_slabs(P.g7, P.g7.groups[gi])));
-  // the shared-layer weight gradient closes the step: balance it over the whole machine
-  ks7[0] = std::max(ks7[0], step_split_critical(step_tiles(P.g7.groups[0]), step_slabs(P.g7, P.g7.groups[0]), sm_count));
-  const int g7 = add_groups(P.g7, ks7);
-  if (g7 < 0) return TA3N_ERR_UNSUPPORTED;
-  const int job0 = (int)B->jobs.size();
-  const int cj = counters((int)P.jobs.size());
-  std::vector<int> job_parts(P.jobs.size(), 0);
-  for (size_t ji = 0; ji < P.jobs.size(); ++ji) {
-    WColsumJob j = P.jobs[ji].job;
-    step_prepare_job(&j);
-    j.partial = carve((size_t)j.nsplit * j.N2 * j.N);
-    job_parts[ji] = ((j.N + 127) / 128) * j.nsplit;
-    B->jobs.push_back(j);
-  }
-  // ================= S6: TRN dgrad per frame (+ frame-disc gradient, ReLU/dropout backward) (spine) =================
-  std::vector<int> ones6(P.g6.groups.size(), 1);
-  const int g6 = add_groups(P.g6, ones6);
-  if (g6 < 0) return TA3N_ERR_UNSUPPORTED;
-  const int c6 = counters(nmb * T);
-  const int c6_total = counters(1);
-  const int need6 = (P.g6.groups[0].N + TC_BN - 1) / TC_BN;
-  {
-    std::vector<StepTask> v;
-    for (int t = 0; t < T; ++t) {
-      // the frame-discriminator gradient this tile accumulates onto lives in frame rows [T m0, T (m0 + 128))
-      // -> second wait range, filled per tile below
-      const size_t first = v.size();
-      if (emit_group(&v, g6 + t, Dep(),
-                     [&](int m0) {
-                       Dep d;
-                       d.b = c5r + (m0 / TC_BM) * R;
-                       d.e = c5r + (m0 / TC_BM + 1) * R;
-                       d.v = need5r;
-                       return d;
-                     },
-                     [=](int mb) { return c6 + mb * T + t; }, c6_total) != 0)
-        return TA3N_ERR_INVALID;
-      for (size_t k = first; k < v.size(); ++k) {
-        const int r0 = T * v[k].m0, r1 = T * std::min(v[k].m0 + TC_BM, M);
-        v[k].wait_begin[1] = c5f + r0 / TC_BM;
-        v[k].wait_end[1] = c5f + (r1 + TC_BM - 1) / TC_BM;
-        v[k].wait_val[1] = need5f;
-      }
-    }
-    sort_by_slabs(&v);
-    std::stable_sort(v.begin(), v.end(), [](const StepTask& a, const StepTask& b) { return a.m0 < b.m0; });   // block-major
-    append(0, v);
-  }
-  // stage-complete conditions
-  auto dep_of = [&](int bit) {
-    switch (bit) {
-      case DEP_FRAME: return one(c4f_total, n_frame_tasks);
-      case DEP_HEADS: return one(c4c_total, n_row_tasks);
-      case DEP_RELBWD: return one(c4e_total, n_row_tasks);
-      case DEP_DZ: return one(c5r_total, nmb * R * need5r);
-      default: return one(c6_total, nmb * T * need6);
-    }
-  };
-  auto set_deps = [&](StepTask* t, int mask) {
-    int r = 0;
-    for (int bit = 1; bit <= DEP_DFEAT; bit <<= 1)
-      if (mask & bit) {
-        if (r >= 2) return -1;
-        const Dep d = dep_of(bit);
-        t->wait_begin[r] = d.b;
-        t->wait_end[r] = d.e;
-        t->wait_val[r] = d.v;
-        ++r;
-      }
-    return 0;
-  };
-  auto emit_jobs = [&](int q, int mask) {
-    for (size_t ji = 0; ji < P.jobs.size(); ++ji) {
-      if (P.jobs[ji].dep != mask) continue;
-      const WColsumJob& j = B->jobs[job0 + ji];
-      for (int cb = 0; cb < (j.N + 127) / 128; ++cb)
-        for (int sp = 0; sp < j.nsplit; ++sp) {
-          StepTask t;
-          memset(&t, 0, sizeof(t));
-          t.signal2 = -1;
-          t.type = TASK_COLSUM_PART;
-          t.group = job0 + (int)ji;
-          t.m0 = cb;
-          t.n0 = sp;
-          if (set_deps(&t, mask) != 0) return -1;
-          t.signal = cj + (int)ji;
-          queue[q].push_back(t);
-        }
-    }
-    for (size_t ji = 0; ji < P.jobs.size(); ++ji) {
-      if (P.jobs[ji].dep != mask) continue;
-      StepTask t;
-      memset(&t, 0, sizeof(t));
-      t.signal = t.signal2 = -1;
-      t.type = TASK_COLSUM_REDUCE;
-      t.group = job0 + (int)ji;
-      t.wait_begin[0] = cj + (int)ji;
-      t.wait_end[0] = cj + (int)ji + 1;
-      t.wait_val[0] = job_parts[ji];
-      queue[q].push_back(t);
-    }
-    return 0;
-  };
-  auto emit_wgrad = [&](int q, int mask) {
-    std::vector<StepTask> v;
-    for (size_t gi = 0; gi < P.g7.groups.size(); ++gi)
-      if (P.g7_dep[gi] == mask) {
-        const Dep d = dep_of(mask);
-        if (emit_group(&v, g7 + (int)gi, d, nullptr, nullptr) != 0) return -1;
-      }
-    sort_by_slabs(&v);
-    append(q, v);
-    return 0;
-  };
-  // fillers in the order their operands complete; the shared layer's gradients close the spine
-  for (int mask : {(int)DEP_FRAME, (int)DEP_HEADS, (int)(DEP_HEADS | DEP_FRAME), (int)DEP_RELBWD, (int)DEP_DZ}) {
-    if ((mask & (mask - 1)) == 0 && emit_wgrad(kFill, mask) != 0) return TA3N_ERR_INVALID;
-    if (emit_jobs(kFill, mask) != 0) return TA3N_ERR_INVALID;
-  }
-  if (emit_wgrad(0, DEP_DFEAT) != 0) return TA3N_ERR_INVALID;
-  if (emit_jobs(0, DEP_DFEAT) != 0) return TA3N_ERR_INVALID;
-  {  // advance the dropout step counter once every reader (S1 epilogues, relpool tasks, the G tiles) is done
-    StepTask t;
-    memset(&t, 0, sizeof(t));
-    t.signal = t.signal2 = -1;
-    t.type = TASK_FINISH;
-    const Dep d = dep_of(DEP_DZ);
-    t.wait_begin[0] = d.b;
-    t.wait_end[0] = d.e;
-    t.wait_val[0] = d.v;
-    queue[kFill].push_back(t);
-  }
-  B->tasks.clear();
-  for (int q = 0; q < kStepQueues; ++q) {
-    B->queue_begin[q] = (int)B->tasks.size();
-    for (StepTask& t : queue[q]) t.urgent = (q >= 1 && q <= kStepQueues - 2) ? 1 : 0;      // the row-block chains
-    B->tasks.insert(B->tasks.end(), queue[q].begin(), queue[q].end());
-  }
-  B->queue_begin[kStepQueues] = (int)B->tasks.size();
-  B->n_counters = nc;
-  B->partial_floats = pused;
-  if (partial_base && pused > partial_cap_floats) return fail(TA3N_ERR_WORKSPACE, "fused step: partial workspace too small");
   return TA3N_OK;
 }
 

@@ -1,6 +1,6 @@
-// step_rows.cuh -- the row ("SIMT") tasks of the fused training step: everything of the path that is not a
-// dense contraction, written as device functions over a group of 256 threads so that they run either as
-// stand-alone kernels (phased executor) or as tasks of the persistent step kernel (step_kernel.cuh).
+// step_rows.cuh -- the row ("SIMT") tasks of the step program: everything of the path that is not a dense
+// contraction, written as device functions over a group of 256 threads, and the kernels that launch them
+// (ta3n_step_run_phased).
 //
 //   frame_task   : per frame row -- frame head models.py:461, its domain loss and gradient main.py:513-538, data
 //                  gradient down to the hidden layer of the frame discriminator.
@@ -73,21 +73,11 @@ struct TailArgs {
   const float* G;                    // [M, H]     d loss / d feat_video (completed by the video-discriminator dgrad GEMM)
   float* dHid;                       // [R, M, H]
   float* dHf;                        // [M*T, F]
-  unsigned long long* dbg;           // development: [M / 8][8] phase timestamps of the relpool / heads tasks (or null)
 };
 
-__device__ __forceinline__ void row_mark(const TailArgs& a, int task, int slot, int warp, int lane) {
-  if (a.dbg && warp == 0 && lane == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    a.dbg[(size_t)task * 8 + slot] = t;
-  }
-}
-
-// The argument blocks of the row tasks live in file-scope shared memory: the tasks are compiled OUT OF LINE (their
-// register allocation stays separate from the GEMM roles of the step kernel, whose 168-register budget they blew as
-// inlined code: 1.6 KB of spills), and a reference to a known __shared__ object keeps every field access an LDS that
-// global stores cannot alias -- passed as `const TailArgs&` the block became generic loads repeated after every store.
+// The argument blocks of the row tasks live in file-scope shared memory, and the tasks are compiled out of line
+// and read them through a reference to that known __shared__ object: every field access stays an LDS that global
+// stores cannot alias.  Passed as `const TailArgs&` the block became generic loads repeated after every store.
 __shared__ TailArgs g_tail;
 __shared__ WColsumJob g_job;
 
@@ -306,7 +296,6 @@ __device__ __noinline__ void relpool_task_t(const int v0, const int nv, const in
   const int lane = tid & 31, warp = tid >> 5;
   const int M = a.M, R = a.R, H = a.H;
   const size_t plane = (size_t)M * H;
-  row_mark(a, v0 / kRowVideos, 0, warp, lane);
   for (int v = warp; v < nv; v += 8) {
     const int m = v0 + v;
     // relation logits from the discriminators' hidden layer -> attention weights; lane i keeps w_i + 1 of scale i.
@@ -354,7 +343,6 @@ __device__ __noinline__ void relpool_task_t(const int v0, const int nv, const in
         if (live && (i & 31) == lane) wp1 = wi + 1.0f;    // R <= 32
       }
     }
-    row_mark(a, v0 / kRowVideos, 1, warp, lane);
     RowVec<HV> y;
 #pragma unroll
     for (int kk = 0; kk < HV; ++kk) y.c[kk] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -401,7 +389,6 @@ __device__ __noinline__ void relpool_task_t(const int v0, const int nv, const in
         }
       }
     }
-    row_mark(a, v0 / kRowVideos, 2, warp, lane);
     row_store<HV>(a.feat_video + (size_t)m * H, lane, y);
 #pragma unroll
     for (int kk = 0; kk < HV; ++kk) {
@@ -421,7 +408,6 @@ __device__ __noinline__ void relpool_task_t(const int v0, const int nv, const in
       }
     }
     row_store<HV>(a.dropped + (size_t)m * H, lane, y);
-    row_mark(a, v0 / kRowVideos, 3, warp, lane);
   }
 }
 
@@ -445,7 +431,6 @@ __device__ __noinline__ void heads_task_t(const int v0, const int nv, const int 
     const int m = v0 + v;
     const int dom = m >= Bs ? 1 : 0;
     const bool real = dom ? (m - Bs < ln.vt) : (m < ln.vs);
-    row_mark(a, v0 / kRowVideos, 4, warp, lane);
     const RowVec<HV> d = row_load_cg<HV>(a.dropped + (size_t)m * H, lane);
     const RowVec<HV> hv = row_load_cg<HV>(a.hid_v + (size_t)m * H, lane);
     const int y_lab = (m < Bs) ? (int)a.labels[m] : -1;    // requested early: off the critical chain below
@@ -490,7 +475,6 @@ __device__ __noinline__ void heads_task_t(const int v0, const int nv, const int 
       a.pred_dom[(size_t)m * 2] = pd0;
       a.pred_dom[(size_t)m * 2 + 1] = pd1;
     }
-    row_mark(a, v0 / kRowVideos, 5, warp, lane);
     // ---- loss heads ----
     float gv[CV];
     float g0 = 0.f, g1 = 0.f, loss = 0.f;
@@ -568,7 +552,6 @@ __device__ __noinline__ void heads_task_t(const int v0, const int nv, const int 
       a.g_dom[(size_t)m * 2 + 1] = g1;
       a.row_loss[m] = loss;
     }
-    row_mark(a, v0 / kRowVideos, 6, warp, lane);
     // ---- dHv = (g_dom W2v) * 1[hid_v > 0]                                                  (head_bwd_data) ----
     RowVec<HV> o;
 #pragma unroll
@@ -598,7 +581,6 @@ __device__ __noinline__ void heads_task_t(const int v0, const int nv, const int 
       }
     }
     row_store<HV>(a.Gc + (size_t)m * H, lane, o);
-    row_mark(a, v0 / kRowVideos, 7, warp, lane);
   }
 }
 
@@ -809,6 +791,47 @@ __device__ __noinline__ void colsum_reduce_task(const int tid) {
     for (; sp < nsplit; ++sp) s += __ldcg(p + (size_t)sp * total);
     j.out[(size_t)(e / j.N) * j.ldo + (e % j.N)] = s;
   }
+}
+
+// ---- stand-alone row kernels of the phased executor --------------------------------------------------------
+__global__ void __launch_bounds__(kRowThreads) frame_row_kernel(const __grid_constant__ TailArgs a) {
+  for (int i = threadIdx.x; i < (int)(sizeof(TailArgs) / sizeof(int)); i += kRowThreads)
+    reinterpret_cast<int*>(&g_tail)[i] = reinterpret_cast<const int*>(&a)[i];
+  __syncthreads();
+  pdl_wait();
+  const int r0 = blockIdx.x * kRowFrames;
+  const int nr = min(kRowFrames, a.M * a.T - r0);
+  if (nr > 0) frame_task(r0, nr, threadIdx.x);
+}
+
+__global__ void __launch_bounds__(kRowThreads) video_row_kernel(const __grid_constant__ TailArgs a, const int kind) {
+  for (int i = threadIdx.x; i < (int)(sizeof(TailArgs) / sizeof(int)); i += kRowThreads)
+    reinterpret_cast<int*>(&g_tail)[i] = reinterpret_cast<const int*>(&a)[i];
+  __syncthreads();
+  pdl_wait();
+  const int v0 = blockIdx.x * kRowVideos;
+  const int nv = min(kRowVideos, a.M - v0);
+  if (nv > 0) video_row_task(kind, v0, nv, threadIdx.x);
+}
+
+// column sums of the phased executor: the same task functions, (job, column block, row split) from the block index
+__global__ void __launch_bounds__(kRowThreads) step_colsum_part_kernel(const __grid_constant__ WColsumTable tab) {
+  __shared__ __align__(16) float red_sm[8 * 33 * 4];
+  pdl_wait();
+  for (int i = threadIdx.x; i < (int)(sizeof(WColsumJob) / sizeof(int)); i += kRowThreads)
+    reinterpret_cast<int*>(&g_job)[i] = reinterpret_cast<const int*>(&tab.job[blockIdx.y])[i];
+  __syncthreads();
+  colsum_part_task(red_sm, blockIdx.x, blockIdx.z, threadIdx.x);
+}
+
+__global__ void __launch_bounds__(kRowThreads)
+step_colsum_reduce_kernel(const __grid_constant__ WColsumTable tab, unsigned long long* step_counter) {
+  pdl_wait();
+  for (int i = threadIdx.x; i < (int)(sizeof(WColsumJob) / sizeof(int)); i += kRowThreads)
+    reinterpret_cast<int*>(&g_job)[i] = reinterpret_cast<const int*>(&tab.job[blockIdx.x])[i];
+  __syncthreads();
+  colsum_reduce_task(threadIdx.x);
+  if (step_counter && blockIdx.x == 0 && threadIdx.x == 0) step_counter[0] += 1ull;   // last launch of the step
 }
 
 }  // namespace ta3n

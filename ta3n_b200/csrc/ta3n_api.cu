@@ -944,40 +944,22 @@ int ta3n_counter_inc(uint64_t* counter, ta3n_stream_t stream) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// the fused training step (include/ta3n_b200.h: ta3n_step_*)
+// the training step (include/ta3n_b200.h: ta3n_step_*)
 // ------------------------------------------------------------------------------------------------
-namespace {
-
-constexpr int kStepMagic = 0x7A3B5700;
-int step_kernel_config(int* sm_count) {          // per-device opt-in of the large dynamic shared memory
-  std::lock_guard<std::mutex> lock(device_mu());
-  DeviceInfo* d = device_info();
-  if (!d) return fail(TA3N_ERR_CUDA, "cudaGetDevice failed");
-  if (!d->step_configured) {
-    TA3N_CUDA(cudaFuncSetAttribute(ta3n_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStepSmemBytes));
-    d->step_configured = true;
-  }
-  *sm_count = d->sm_count;
-  return TA3N_OK;
-}
-
-}  // namespace
-
 size_t ta3n_step_workspace_bytes(const ta3n_step_desc* desc) {
   StepProgram P;
   if (build_step_program(desc, &P, /*dry=*/true) != TA3N_OK) return 0;
-  BuiltPlan B;
-  if (build_task_graph(P, device_sm_count(), nullptr, 0, &B) != TA3N_OK) return 0;
-  // column-sum partials of the phased executor use the same job preparation -> covered by partial_floats
-  return P.scratch_bytes + Arena::round(B.partial_floats * sizeof(float)) + 4096;
+  // the column-sum partials follow the fixed scratch: carved by the same walk as in ta3n_step_run_phased, from an
+  // arena that only hands out addresses (nothing is dereferenced)
+  Arena partials(reinterpret_cast<void*>(uintptr_t(1) << 20), size_t(1) << 46);
+  if (step_colsum_batches(P, &partials, [](const WColsumTable&, bool) { return TA3N_OK; }) != TA3N_OK) return 0;
+  return P.scratch_bytes + partials.used;
 }
 
 int ta3n_step_run_phased(const ta3n_step_desc* desc, ta3n_stream_t stream) {
   StepProgram P;
   TA3N_TRY(build_step_program(desc, &P));
   cudaStream_t st = S(stream);
-  int sm_count = 132;
-  TA3N_TRY(step_kernel_config(&sm_count));
   const int n_row = (P.M + kRowVideos - 1) / kRowVideos;
   auto rows = [&](const char* label, int kind) {
     pre_launch(label, st);
@@ -998,126 +980,22 @@ int ta3n_step_run_phased(const ta3n_step_desc* desc, ta3n_stream_t stream) {
   TA3N_TRY(run_gemm(P.g5, st));
   TA3N_TRY(run_gemm(P.g6, st));
   TA3N_TRY(run_gemm(P.g7, st));
-  // column sums: parts, then the fixed-order reduction (which also advances the dropout step counter)
+  // column sums: parts, then the fixed-order reduction (whose last launch also advances the dropout step counter)
   Arena arena(static_cast<char*>(desc->workspace) + P.scratch_bytes, desc->workspace_bytes - P.scratch_bytes);
-  size_t i = 0;
-  bool counter_done = desc->step_counter == nullptr;
-  while (i < P.jobs.size()) {
-    WColsumTable tab;
-    tab.n_jobs = 0;
+  return step_colsum_batches(P, &arena, [&](const WColsumTable& tab, bool last) {
     int max_cb = 1, max_split = 1;
-    while (i < P.jobs.size() && tab.n_jobs < kMaxWColsumJobs) {
-      WColsumJob j = P.jobs[i].job;
-      step_prepare_job(&j);
-      j.partial = arena.floats((size_t)j.nsplit * j.N2 * j.N);
-      if (!j.partial) return fail(TA3N_ERR_WORKSPACE, "fused step: column-sum workspace too small");
-      max_cb = std::max(max_cb, (j.N + 127) / 128);
-      max_split = std::max(max_split, j.nsplit);
-      tab.job[tab.n_jobs++] = j;
-      ++i;
+    for (int k = 0; k < tab.n_jobs; ++k) {
+      max_cb = std::max(max_cb, (tab.job[k].N + 127) / 128);
+      max_split = std::max(max_split, tab.job[k].nsplit);
     }
     pre_launch("step_colsum", st);
     launch_kernel(step_colsum_part_kernel, dim3(max_cb, tab.n_jobs, max_split), kRowThreads, 0, st, tab);
     TA3N_TRY(after_launch());
-    const bool last = i >= P.jobs.size();
     pre_launch("step_colsum_reduce", st);
     launch_kernel(step_colsum_reduce_kernel, tab.n_jobs, kRowThreads, 0, st, tab,
-                  reinterpret_cast<unsigned long long*>((last && !counter_done) ? desc->step_counter : nullptr));
-    TA3N_TRY(after_launch());
-    if (last) counter_done = true;
-  }
-  return TA3N_OK;
-}
-
-namespace {
-struct PlanLayout {
-  size_t tasks, groups, segs, maps, jobs, tail, counters, total;
-};
-PlanLayout plan_layout(const BuiltPlan& B) {
-  PlanLayout l;
-  size_t off = 0;
-  auto put = [&](size_t bytes) {
-    const size_t at = off;
-    off += (bytes + 255) & ~size_t(255);
-    return at;
-  };
-  l.maps = put(B.maps.size() * sizeof(CUtensorMap));
-  l.tasks = put(B.tasks.size() * sizeof(StepTask));
-  l.groups = put(B.groups.size() * sizeof(StepGroup));
-  l.segs = put(B.segs.size() * sizeof(SegLite));
-  l.jobs = put(B.jobs.size() * sizeof(WColsumJob));
-  l.tail = put(sizeof(TailArgs));
-  l.counters = put((size_t)(B.n_counters + kStepQueues) * sizeof(int));
-  l.total = off;
-  return l;
-}
-}  // namespace
-
-size_t ta3n_step_plan_bytes(const ta3n_step_desc* desc) {
-  StepProgram P;
-  if (build_step_program(desc, &P, /*dry=*/true) != TA3N_OK) return 0;
-  BuiltPlan B;
-  if (build_task_graph(P, device_sm_count(), nullptr, 0, &B) != TA3N_OK) return 0;
-  return plan_layout(B).total + 1024;
-}
-
-int ta3n_step_build(const ta3n_step_desc* desc, void* plan_dev, size_t plan_bytes, void* handle_host) {
-  TA3N_REQUIRE(plan_dev != nullptr && handle_host != nullptr, "null plan / handle");
-  TA3N_REQUIRE((reinterpret_cast<uintptr_t>(plan_dev) & 255u) == 0, "plan buffer must be 256-byte aligned");
-  StepProgram P;
-  TA3N_TRY(build_step_program(desc, &P));
-  int sm_count = 132;
-  TA3N_TRY(step_kernel_config(&sm_count));
-  BuiltPlan B;
-  float* partial = reinterpret_cast<float*>(static_cast<char*>(desc->workspace) + P.scratch_bytes);
-  const size_t partial_cap = (desc->workspace_bytes - P.scratch_bytes) / sizeof(float);
-  TA3N_TRY(build_task_graph(P, sm_count, partial, partial_cap, &B));
-  const PlanLayout l = plan_layout(B);
-  if (l.total > plan_bytes) return fail(TA3N_ERR_WORKSPACE, "ta3n_step_build: plan buffer too small (%zu < %zu)", plan_bytes, l.total);
-  std::vector<char> host(l.total, 0);
-  memcpy(host.data() + l.maps, B.maps.data(), B.maps.size() * sizeof(CUtensorMap));
-  memcpy(host.data() + l.tasks, B.tasks.data(), B.tasks.size() * sizeof(StepTask));
-  memcpy(host.data() + l.groups, B.groups.data(), B.groups.size() * sizeof(StepGroup));
-  memcpy(host.data() + l.segs, B.segs.data(), B.segs.size() * sizeof(SegLite));
-  memcpy(host.data() + l.jobs, B.jobs.data(), B.jobs.size() * sizeof(WColsumJob));
-  memcpy(host.data() + l.tail, &P.tail, sizeof(TailArgs));
-  TA3N_CUDA(cudaMemcpy(plan_dev, host.data(), l.total, cudaMemcpyHostToDevice));
-  char* base = static_cast<char*>(plan_dev);
-  StepHandle h;
-  memset(&h, 0, sizeof(h));
-  h.hd.n_tasks = (int)B.tasks.size();
-  h.hd.n_counters = B.n_counters;
-  h.hd.n_groups = (int)B.groups.size();
-  h.hd.n_jobs = (int)B.jobs.size();
-  h.hd.tasks = reinterpret_cast<const StepTask*>(base + l.tasks);
-  h.hd.groups = reinterpret_cast<const StepGroup*>(base + l.groups);
-  h.hd.segs = reinterpret_cast<const SegLite*>(base + l.segs);
-  h.hd.maps = reinterpret_cast<const CUtensorMap*>(base + l.maps);
-  h.hd.jobs = reinterpret_cast<const WColsumJob*>(base + l.jobs);
-  h.hd.tail = reinterpret_cast<const TailArgs*>(base + l.tail);
-  h.hd.counters = reinterpret_cast<int*>(base + l.counters);
-  h.hd.step_counter = reinterpret_cast<unsigned long long*>(desc->step_counter);
-  for (int q = 0; q <= kStepQueues; ++q) h.hd.queue_begin[q] = B.queue_begin[q];
-  h.magic = kStepMagic;
-  h.n_gemm_tiles = B.n_gemm_tiles;
-  h.smem_bytes = kStepSmemBytes;
-  h.grid = sm_count;
-  memset(handle_host, 0, TA3N_STEP_HANDLE_BYTES);
-  memcpy(handle_host, &h, sizeof(h));
-  return TA3N_OK;
-}
-
-int ta3n_step_run(const void* handle_host, ta3n_stream_t stream) {
-  TA3N_REQUIRE(handle_host != nullptr, "null handle");
-  StepHandle h;
-  memcpy(&h, handle_host, sizeof(h));
-  TA3N_REQUIRE(h.magic == kStepMagic, "not a handle filled by ta3n_step_build");
-  cudaStream_t st = S(stream);
-  // arrival counters and the queues' ticket cursors
-  TA3N_CUDA(cudaMemsetAsync(h.hd.counters, 0, (size_t)(h.hd.n_counters + kStepQueues) * sizeof(int), st));
-  pre_launch("step_kernel", st);
-  ta3n_step_kernel<<<h.grid, kStepThreads, h.smem_bytes, st>>>(h.hd);
-  return after_launch();
+                  reinterpret_cast<unsigned long long*>(last ? desc->step_counter : nullptr));
+    return after_launch();
+  });
 }
 
 // Host-only: the split-K factors the balanced planner (gemm_wgmma.cuh: plan_splitk_balanced) would choose for a
@@ -1146,98 +1024,6 @@ int ta3n_plan_forward_splits(int n_groups, const int* M, const int* N, const int
     makespan_out[0] = before;
     makespan_out[1] = x3_makespan(plan, ks, sms);
   }
-  return TA3N_OK;
-}
-
-// Host-only description of the task graph the fused step would run for `desc` (no CUDA call; pointers in desc only
-// need to be non-null): "tasks T gemm_tiles G tail R colsum_parts P colsum_reduces Q counters N maps K slabs S".
-size_t ta3n_step_describe(const ta3n_step_desc* desc, char* buf, size_t buf_bytes) {
-  StepProgram P;
-  if (build_step_program(desc, &P, /*dry=*/true) != TA3N_OK) return 0;
-  BuiltPlan B;
-  if (build_task_graph(P, 132, nullptr, 0, &B) != TA3N_OK) return 0;
-  int n_type[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  long slabs = 0;
-  int bad = 0;
-  // The queue orders must be consistent with the dependencies: a scheduler that only sees the head of every queue has
-  // to be able to finish (also proves that every awaited count is reached and the graph is acyclic).
-  std::vector<int> total(B.n_counters, 0);
-  for (const StepTask& t : B.tasks) {
-    n_type[t.type]++;
-    if (t.type == TASK_GEMM) {
-      const StepGroup& sg = B.groups[t.group];
-      int n = 0;
-      for (int k = 0; k < sg.g.seg_count; ++k) n += (B.segs[sg.seg_begin + k].len + TC_BK - 1) / TC_BK;
-      slabs += (n + sg.g.ksplit - 1) / sg.g.ksplit;
-    }
-    if (t.signal >= 0) total[t.signal]++;
-    if (t.signal2 >= 0) total[t.signal2]++;
-  }
-  {
-    std::vector<int> cnt(B.n_counters, 0);
-    int cur[kStepQueues];
-    for (int q = 0; q < kStepQueues; ++q) cur[q] = B.queue_begin[q];
-    size_t left = B.tasks.size();
-    bool progress = true;
-    while (left > 0 && progress) {      // a scheduler that only ever sees the head of each queue
-      progress = false;
-      for (int q = 0; q < kStepQueues; ++q) {
-        while (cur[q] < B.queue_begin[q + 1]) {
-          const StepTask& t = B.tasks[cur[q]];
-          bool ready = true;
-          for (int r = 0; r < 2 && ready; ++r)
-            for (int c = t.wait_begin[r]; c < t.wait_end[r]; ++c)
-              if (c < 0 || c >= B.n_counters || cnt[c] < t.wait_val[r]) {
-                ready = false;
-                break;
-              }
-          if (!ready) break;
-          ++cur[q];
-          --left;
-          progress = true;
-          bool publish = true;
-          if (t.type == TASK_GEMM && t.mode == TILE_SPLIT)      // only the last split to arrive announces the tile
-            publish = ++cnt[t.split_counter] == B.groups[t.group].g.ksplit;
-          if (publish && t.signal >= 0) cnt[t.signal]++;
-          if (publish && t.signal2 >= 0) cnt[t.signal2]++;
-        }
-      }
-    }
-    bad = (int)left;
-  }
-  char line[512];
-  snprintf(line, sizeof(line),
-           "tasks %zu gemm_tiles %d row %d frame %d colsum_parts %d colsum_reduces %d counters %d maps %zu groups %zu slabs %ld "
-           "partial_floats %zu unsatisfiable_waits %d",
-           B.tasks.size(), n_type[TASK_GEMM], n_type[TASK_ROW], n_type[TASK_FRAME], n_type[TASK_COLSUM_PART],
-           n_type[TASK_COLSUM_REDUCE], B.n_counters, B.maps.size(), B.groups.size(), slabs, B.partial_floats, bad);
-  const size_t n = strlen(line);
-  if (buf && buf_bytes > 0) {
-    const size_t c = n < buf_bytes - 1 ? n : buf_bytes - 1;
-    memcpy(buf, line, c);
-    buf[c] = 0;
-  }
-  return n;
-}
-
-int ta3n_step_set_trace(void* handle_host, unsigned long long* trace_dev) {
-  TA3N_REQUIRE(handle_host != nullptr, "null handle");
-  StepHandle h;
-  memcpy(&h, handle_host, sizeof(h));
-  TA3N_REQUIRE(h.magic == kStepMagic, "not a handle filled by ta3n_step_build");
-  h.hd.trace = trace_dev;
-  memcpy(handle_host, &h, sizeof(h));
-  return TA3N_OK;
-}
-
-int ta3n_step_info(const void* handle_host, int* n_tasks, int* n_counters, int* n_gemm_tiles) {
-  TA3N_REQUIRE(handle_host != nullptr, "null handle");
-  StepHandle h;
-  memcpy(&h, handle_host, sizeof(h));
-  TA3N_REQUIRE(h.magic == kStepMagic, "not a handle filled by ta3n_step_build");
-  if (n_tasks) *n_tasks = h.hd.n_tasks;
-  if (n_counters) *n_counters = h.hd.n_counters;
-  if (n_gemm_tiles) *n_gemm_tiles = h.n_gemm_tiles;
   return TA3N_OK;
 }
 

@@ -111,10 +111,9 @@ class TrainStep:
                  allreduce: Optional[str] = None):
         """mode: 'legacy' (default) = the per-operator sequence (25 launches in one CUDA graph; the only mode that
         supports use_attn_frame); 'phased' = the step program as 14 launches (ta3n_step_run_phased; default when class /
-        domain weights or a scheduled beta are given); 'fused' = the same program as ONE persistent kernel (C ABI
-        ta3n_step_build / ta3n_step_run; plain tf32 tiles whatever engine is selected).  class_weight / domain_weight: the weights of criterion / criterion_domain
-        (main.py:160-167, 204-205; fused and phased modes).  A negative beta entry selects the DANN schedule for that
-        level (main.py:350-352): call set_progress(p) every step.
+        domain weights or a scheduled beta are given).  class_weight / domain_weight: the weights of criterion /
+        criterion_domain (main.py:160-167, 204-205; phased mode).  A negative beta entry selects the DANN schedule for
+        that level (main.py:350-352): call set_progress(p) every step.
         allreduce (world > 1): 'peer' = this library's one-kernel all-reduce over NVLink peer / NVSwitch multicast
         memory (csrc/allreduce.cuh; the gradient bucket then lives in symmetric memory and the whole iteration --
         step, all-reduce, optimizer -- is one CUDA graph), 'nccl' = torch.distributed all_reduce between graphs;
@@ -151,16 +150,15 @@ class TrainStep:
         if mode is None:
             # 'legacy' (the per-operator sequence) is the fastest executor measured so far and honours the selected
             # GEMM engine (DESIGN 4.4); the features only the step program has (class / domain weights, the DANN beta
-            # schedule) select 'phased', which honours the engine too.  'fused' (one persistent kernel, plain tf32
-            # tiles only) is opt-in.
+            # schedule) select 'phased', which honours the engine too.
             needs_step = class_weight is not None or any(float(b) < 0 for b in beta) or \
                 tuple(float(w) for w in domain_weight) != (1.0, 1.0)
             mode = "phased" if (needs_step and model.use_attn_frame == "none") else "legacy"
             mode = os.environ.get("TA3N_STEP_MODE", mode)
-        if mode not in ("fused", "phased", "legacy"):
+        if mode not in ("phased", "legacy"):
             raise ValueError(f"unknown TrainStep mode {mode!r}")
         if mode != "legacy" and model.use_attn_frame != "none":
-            raise NotImplementedError("the fused step does not cover use_attn_frame; use mode='legacy'")
+            raise NotImplementedError("the step program does not cover use_attn_frame; use mode='legacy'")
         if overlap_wgrad is None:
             # measured at cfg2 (tools/legacy_options.py): the weight-gradient launches on a forked stream of the graph
             # gain 12 us per step under the tf32x3 engine (its small precise launch overlaps the data-gradient chain)
@@ -168,14 +166,14 @@ class TrainStep:
             overlap_wgrad = mode == "legacy" and _lib.get_gemm_engine() == "tf32x3" and not overlap_allreduce
         if mode != "legacy" and (overlap_wgrad or parallel_branches or overlap_allreduce or graph_collectives):
             raise ValueError("overlap_wgrad / parallel_branches / overlap_allreduce / graph_collectives are options "
-                             "of mode='legacy' (the fused step is a single kernel)")
+                             "of mode='legacy' (the step program runs its launches on one stream)")
         self.mode = mode
         self.beta_spec = [float(b) for b in beta]
         if mode == "legacy" and any(b < 0 for b in self.beta_spec):
-            raise ValueError("negative beta (= DANN schedule, main.py:350-352) needs mode='fused' or 'phased': the "
+            raise ValueError("negative beta (= DANN schedule, main.py:350-352) needs mode='phased': the "
                              "legacy sequence bakes beta into the captured graph")
         if class_weight is not None and mode == "legacy":
-            raise ValueError("class_weight needs mode='fused' or 'phased'")
+            raise ValueError("class_weight needs mode='phased'")
         self._overlap_requested = bool(overlap_allreduce)
         self.split = (self.world > 1) if overlap_allreduce is None else bool(overlap_allreduce)
         if model.use_attn_frame != "none" or mode != "legacy":
@@ -255,7 +253,7 @@ class TrainStep:
         # independent dropout masks per data-parallel rank, like the reference's DataParallel replicas
         rank = dist.get_rank(process_group) if dist.is_initialized() else 0
         seed = (int(seed) ^ (rank * 0x9E3779B97F4A7C15)) & (2 ** 63 - 1)
-        # GRL coefficients in device memory (fused / phased): rescheduled per step without re-capturing
+        # GRL coefficients in device memory (phased): rescheduled per step without re-capturing
         self.beta_dev = torch.tensor([max(b, 0.0) for b in self.beta_spec], device=dev, dtype=torch.float32)
         self._beta_host = torch.tensor([max(b, 0.0) for b in self.beta_spec], dtype=torch.float32).pin_memory()
         self.class_weight = None if class_weight is None else \
@@ -279,8 +277,7 @@ class TrainStep:
         self.launches_per_step = 0               # kernels of libta3n_sm90.so per step (counted at capture)
         self.use_graph = bool(use_graph)
         self.graphs = [None] * self.n_slots      # per input slot: (graph_a, graph_b or None)
-        self.step_descs = [None] * self.n_slots  # fused / phased: ta3n_step_desc per input slot (+ keep-alives)
-        self.step_handles = [None] * self.n_slots
+        self.step_descs = [None] * self.n_slots  # phased: ta3n_step_desc per input slot (+ keep-alives)
         if self.mode != "legacy":
             for slot in range(self.n_slots):
                 self._build_step(slot)
@@ -346,9 +343,9 @@ class TrainStep:
             _lib.ptr_array([p + slot * self._ar_flag_bytes for p in a["flags"]]), _P(self.step_counter),
             a["rank"], a["world"], hi - lo, stream if stream is not None else TF._stream()))
 
-    # -- the fused step (C ABI ta3n_step_*) ------------------------------------------------------------
+    # -- the step program (C ABI ta3n_step_*) ----------------------------------------------------------
     def _build_step(self, slot):
-        """Describe the step for input slot `slot` (ta3n_step_desc) and, in fused mode, build its task graph."""
+        """Describe the step for input slot `slot` (ta3n_step_desc)."""
         lib = _lib.load()
         xs, xt, labels, valid = self.slots[slot]
         R, M, T = self.R, self.M, self.T
@@ -405,37 +402,14 @@ class TrainStep:
         d.workspace, d.workspace_bytes = _P(ws), ws.numel()
         self.step_descs[slot] = (d, keep, rs)
         self.step_bufs = bufs
-        if self.mode == "fused":
-            plan = self.bufs.workspace(f"step_plan{slot}", lib.ta3n_step_plan_bytes(C.byref(d)))
-            handle = C.create_string_buffer(_lib.STEP_HANDLE_BYTES)
-            check(lib.ta3n_step_build(C.byref(d), _P(plan), plan.numel(), handle))
-            self.step_handles[slot] = handle
         self.outputs = (bufs["feat"].view(M, T, F), bufs["pred_frame"].view(M, T, 2), bufs["attn"], bufs["pred_rel"],
                         bufs["feat_video"], bufs["pred_video"], bufs["pred_dom"])
 
-    def step_info(self):
-        """(tasks, arrival counters, GEMM tiles) of the fused step's task graph."""
-        n = [C.c_int(), C.c_int(), C.c_int()]
-        check(_lib.load().ta3n_step_info(self.step_handles[self.active], *[C.byref(x) for x in n]))
-        return tuple(x.value for x in n)
-
-    def trace(self, enable: bool = True):
-        """Fused mode, eager or before capture: record {SM, scheduled, accumulator ready, done} per task of the step
-        kernel (ta3n_step_set_trace).  Returns the device tensor (n_tasks, 8) int64 the kernel fills."""
-        lib = _lib.load()
-        n_tasks = self.step_info()[0]
-        if not hasattr(self, "_trace_buf"):
-            self._trace_buf = torch.zeros(n_tasks + (self.M + 7) // 8, 8, device=self.device, dtype=torch.int64)
-        for h in self.step_handles:
-            if h is not None:
-                check(lib.ta3n_step_set_trace(h, _P(self._trace_buf) if enable else None))
-        return self._trace_buf
-
     def set_beta(self, beta: Sequence[float]):
-        """New GRL coefficients {relation, video, frame} for the following steps (fused / phased modes): one
-        12-byte async copy, no re-capture."""
+        """New GRL coefficients {relation, video, frame} for the following steps (phased mode): one 12-byte async
+        copy, no re-capture."""
         if self.mode == "legacy":
-            raise ValueError("set_beta needs mode='fused' or 'phased'")
+            raise ValueError("set_beta needs mode='phased'")
         for i in range(3):
             self._beta_host[i] = float(beta[i])
         self.beta_dev.copy_(self._beta_host, non_blocking=True)
@@ -494,10 +468,7 @@ class TrainStep:
 
     def _enqueue_body(self, lib, st, at_split, optimizer):
         if self.mode != "legacy":
-            if self.mode == "fused":
-                check(lib.ta3n_step_run(self.step_handles[self.active], st))
-            else:
-                check(lib.ta3n_step_run_phased(C.byref(self.step_descs[self.active][0]), st))
+            check(lib.ta3n_step_run_phased(C.byref(self.step_descs[self.active][0]), st))
             if self.ar is not None:
                 self._enqueue_allreduce()         # same stream, same graph: step -> all-reduce -> optimizer
             if optimizer and self.opt is not None:

@@ -36,9 +36,15 @@ def test_every_declared_symbol_is_exported(lib):
         assert hasattr(raw, name), f"{name} declared in the header but not exported"
 
 
-def test_abi_version_and_engine_switch(lib):
+def test_abi_version_matches_header(lib):
+    """The library, the header and the binding agree on the ABI version (bumped whenever a symbol goes)."""
     from ta3n_b200 import _lib
-    assert lib.ta3n_abi_version() == 2
+    header = int(re.search(r"#define\s+TA3N_ABI_VERSION\s+(\d+)", open(HEADER).read()).group(1))
+    assert lib.ta3n_abi_version() == header == _lib.ABI_VERSION
+
+
+def test_engine_switch(lib):
+    from ta3n_b200 import _lib
     assert _lib.get_gemm_engine() == "tf32x3"          # the library default: the parity-tested product engine
     _lib.set_gemm_engine("tf32")
     assert _lib.get_gemm_engine() == "tf32"
