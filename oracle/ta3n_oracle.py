@@ -226,16 +226,25 @@ def _relu(x: torch.Tensor, gate: Optional[torch.Tensor]) -> torch.Tensor:
     return F.relu(x) if gate is None else x * gate.to(x.dtype)
 
 
-def activation_pattern(params, xs, xt, beta, cfg: "PathConfig") -> Dict[str, torch.Tensor]:
-    """The ReLU on/off pattern of a plain (dropout-free) oracle forward, in the ``gates`` format
-    (M = Bs+Bt rows, source first) -- used to test the gate plumbing against itself."""
+def activation_pattern(params, xs, xt, beta, cfg: "PathConfig",
+                       masks: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
+    """The ReLU on/off pattern of an oracle training forward, in the ``gates`` format (M = Bs+Bt rows, source
+    first).  Without ``masks`` the forward is dropout-free; with keep masks (the ``forward`` format) dropout_i /
+    dropout_v act at cfg's rates, as in ``forward(train=True, masks=masks)``.  'shared' is the sign of the shared
+    layer's pre-activation, which dropout does not change."""
     p = params
     T, Fd, R = cfg.num_segments, cfg.shared_dim, cfg.num_segments - 1
     tuples = relation_tuples(T)
     x = torch.cat([xs, xt], 0)
     M = x.size(0)
+    mask_i = mask_v = None
+    if masks:
+        mask_i = torch.cat([masks["i_source"], masks["i_target"]], 0) if "i_source" in masks else None
+        mask_v = torch.cat([masks["v_source"], masks["v_target"]], 0) if "v_source" in masks else None
     pre = F.linear(x.reshape(-1, x.size(-1)), p["fc_feature_shared_source.weight"], p["fc_feature_shared_source.bias"])
     feat = F.relu(pre)
+    if mask_i is not None:
+        feat = _apply_dropout(feat, cfg.dropout_i, True, mask_i)
     hf = F.linear(feat, p["fc_feature_domain.weight"], p["fc_feature_domain.bias"])
     g = {"shared": pre > 0, "frame_disc": hf > 0}
     if cfg.use_attn_frame != "none":
@@ -264,6 +273,8 @@ def activation_pattern(params, xs, xt, beta, cfg: "PathConfig") -> Dict[str, tor
         w = entropy_attention(pr.reshape(-1, 2)).view(M, R)
         relf = (w.unsqueeze(-1) + 1) * relf
     vid = relf.sum(1)
+    if mask_v is not None:
+        vid = _apply_dropout(vid, cfg.dropout_v, True, mask_v)
     g["video_disc"] = F.linear(vid, p["fc_feature_domain_video.weight"], p["fc_feature_domain_video.bias"]) > 0
     return g
 

@@ -490,8 +490,8 @@ def test_single_video_and_empty_target():
 
 
 def test_in_kernel_dropout_statistics_and_mask_consistency():
-    """Perf-mode dropout (counter-based RNG): keep rate ~ 1-p, scaling 1/(1-p), fresh mask per call,
-    and backward uses the same mask as forward (gradient is zero exactly where the feature is zero)."""
+    """Perf-mode dropout (counter-based RNG): keep rate ~ 1-p, scaling 1/(1-p), fresh mask per call.  The masks
+    themselves, and that backward uses the forward's mask, are checked exactly in tests/test_dropout_rng.py."""
     cfg = orc.PathConfig(num_class=12, num_segments=5, fc_dim=512, dropout_i=0.5, dropout_v=0.5)
     params = orc.init_params(cfg, seed=1234)
     model = build_model(cfg, params, train=True)
