@@ -970,24 +970,32 @@ inline bool tc_operand_ok(const float* p, int ld) {
   return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15u) == 0 && (ld % 4) == 0 && ld > 0;
 }
 
-// Is this group worth / able to run on the tensor-core engine?
-inline bool tc_group_ok(const GemmPlan& plan, const Group& g) {
-  if (plan.load_flags != 0) return false;                    // ReLU-on-load needs a register pass
-  if ((long)g.M * g.N < 64L * 64L) return false;             // tiny heads stay on the SIMT engine
-  if (g.seg_count > kMaxSegs) return false;
-  for (int i = 0; i < g.seg_count; ++i) {
-    const Seg& s = plan.segs[g.seg_begin + i];
-    if (!tc_operand_ok(s.A, s.lda) || !tc_operand_ok(s.B, s.ldb) || s.len <= 0) return false;
-  }
-  return true;
-}
-
-// tensor-map keys of one segment of a group (shared by the per-launch and the step-kernel planners)
+// tensor-map keys of one segment of a group (launch_tc deduplicates them within a launch)
 inline void tc_seg_keys(const Seg& s, const Group& g, bool a_kmaj, bool b_kmaj, bool a3d, bool b3d, MapKey* ka,
                         MapKey* kb, bool raw = false) {
   const int rw = raw ? 1 : 0;
   *ka = a_kmaj ? MapKey{s.A, s.len, g.M, s.lda, TC_BK, TC_BM, 0, rw} : MapKey{s.A, g.M, s.len, s.lda, 32, TC_BK, a3d ? 1 : 0, rw};
   *kb = b_kmaj ? MapKey{s.B, s.len, g.N, s.ldb, TC_BK, TC_BN, 0, rw} : MapKey{s.B, g.N, s.len, s.ldb, 32, TC_BK, b3d ? 1 : 0, rw};
+}
+
+// Is this group worth / able to run on the tensor-core engine?
+inline bool tc_group_ok(const GemmPlan& plan, const Group& g) {
+  if (plan.load_flags != 0) return false;                    // ReLU-on-load needs a register pass
+  if ((long)g.M * g.N < 64L * 64L) return false;             // tiny heads stay on the SIMT engine
+  if (g.seg_count > kMaxSegs) return false;
+  std::map<MapKey, int> maps;
+  for (int i = 0; i < g.seg_count; ++i) {
+    const Seg& s = plan.segs[g.seg_begin + i];
+    if (!tc_operand_ok(s.A, s.lda) || !tc_operand_ok(s.B, s.ldb) || s.len <= 0) return false;
+    // the rank-3 and raw flags are the same for every segment of a launch: they do not change the count
+    MapKey ka, kb;
+    tc_seg_keys(s, g, plan.a_kmaj, plan.b_kmaj, false, false, &ka, &kb);
+    maps[ka] = maps[kb] = 0;
+  }
+  // the maps of one launch sit in its kernel parameters: a group that needs more of them than one launch holds
+  // (the data gradient of a frame of a long clip: one A and one B map per relation slot reading it) runs on the SIMT
+  // engine
+  return (int)maps.size() <= kMaxMaps;
 }
 
 template <bool A_KMAJ, bool B_KMAJ>

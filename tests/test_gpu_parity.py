@@ -114,7 +114,8 @@ def test_model_matches_reference_golden(case, engine):
 # ------------------------------------------------------------------------------------------------
 # live oracle at a mid size with non-degenerate (trained-like) weights
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("T,attn_frame,bs,bt", [(5, "none", 37, 21), (7, "TransAttn", 16, 16)])
+@pytest.mark.parametrize("T,attn_frame,bs,bt", [(5, "none", 37, 21), (7, "TransAttn", 16, 16), (10, "TransAttn", 7, 6),
+                                                (20, "none", 12, 10)])
 def test_model_matches_oracle_mid_size(T, attn_frame, bs, bt, engine):
     cfg = orc.PathConfig(num_class=12, num_segments=T, fc_dim=512, dropout_i=0.5, dropout_v=0.5,
                          use_attn="TransAttn", use_attn_frame=attn_frame)
@@ -319,7 +320,7 @@ def test_tf32_gradients_match_oracle_on_realised_activation_pattern(T, attn_fram
 # ------------------------------------------------------------------------------------------------
 # stand-alone RelationModuleMultiScale (negative inputs exercise the leading ReLU, TRNmodule.py:49)
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("T,F,N", [(5, 64, 9), (3, 128, 70), (9, 32, 5), (2, 16, 3)])
+@pytest.mark.parametrize("T,F,N", [(5, 64, 9), (3, 128, 70), (9, 32, 5), (2, 16, 3), (20, 64, 70)])
 def test_trn_module_matches_oracle(T, F, N, engine):
     from ta3n_b200.TRNmodule import RelationModuleMultiScale
     torch.manual_seed(3)
@@ -547,7 +548,8 @@ def test_cpu_tensors_are_moved_not_computed_on_cpu():
 @pytest.mark.parametrize("mode", ["legacy", "phased"])
 @pytest.mark.parametrize("use_graph", [False, True])
 @pytest.mark.parametrize("T,attn_frame,bs,bt,C", [(5, "none", 24, 24, 12), (4, "TransAttn", 9, 5, 30),
-                                                   (3, "none", 60, 11, 51)])     # C > 32: chunked class head
+                                                   (3, "none", 60, 11, 51),      # C > 32: chunked class head
+                                                   (20, "none", 8, 8, 12)])      # long clip: TRN groups of > 64 maps
 def test_fused_train_step_matches_oracle(T, attn_frame, bs, bt, C, use_graph, engine, mode):
     """TrainStep (forward + fused loss heads + backward, no autograd) vs the fp64 oracle's
     loss and parameter gradients; dropout off so both see the same function.  Both executors: the per-operator
