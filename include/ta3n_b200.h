@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define TA3N_ABI_VERSION 3
+#define TA3N_ABI_VERSION 4
 
 enum {
   TA3N_OK = 0,
@@ -210,7 +210,8 @@ size_t ta3n_video_head_bwd_workspace_bytes(int M, int H, int C);
 /* g_pred [M,C] (may be NULL), d_dropped_extra [M,H] = gradient already accumulated on the
  * dropped features by the video discriminator (may be NULL), g_feat_video_ext [M,H] (may be
  * NULL).  grad_scale multiplies everything that flows through the optional GRL_mu
- * (reverse ? -mu : 1).  Produces d_feat_video [M,H], dWc [C,H], dbc [C].                 */
+ * (reverse ? -mu : 1).  Produces d_feat_video [M,H], dWc [C,H], dbc [C].  d_feat_video may be
+ * NULL: only the weight / bias gradient is computed (MCD's reverse pass with mu == 0).   */
 int ta3n_video_head_bwd(const float* dropped, int M, int H, int C, const float* Wc,
                         const ta3n_dropout* drop, const float* g_pred,
                         const float* d_dropped_extra, const float* g_feat_video_ext,
@@ -254,6 +255,26 @@ int ta3n_loss_fwd_bwd(const float* pred_video, const long long* labels, const fl
                       void* workspace, size_t workspace_bytes, ta3n_stream_t stream);
 /* *counter += 1 on the stream (dropout step counter for CUDA-graph replays). */
 int ta3n_counter_inc(uint64_t* counter, ta3n_stream_t stream);
+
+/* ---- loss terms of ens_DA='MCD' (main.py:446-448, 548-556; loss.py:29-30) ------------------------------------- */
+/* Both are one single-block launch whose rows are summed in a fixed order, so that graph replays give bit-identical
+ * losses; both ADD to *loss.  rows == 0 is a no-op.  valid_rows (device, optional) is the {real source rows, real
+ * target rows} pair of ta3n_loss_fwd_bwd: padded rows get zero gradient and the means run over the real rows.
+ *
+ * Class CE of the second classifier on the source rows (main.py:447-448):
+ *   loss += mean over r < valid_rows[0] of CE(pred[r], labels[r]);  g_pred [rows,C] = its gradient.             */
+int ta3n_ce_loss_fwd_bwd(const float* pred, const long long* labels, int rows, int C, const int* valid_rows,
+                         float* loss, float* g_pred, ta3n_stream_t stream);
+/* Classifier discrepancy of the reverse pass on the target rows (main.py:548-556):
+ *   loss += -mean |softmax(pred1) - softmax(pred2)| over r < valid_rows[1] and the C classes
+ * (0 when there is no real row); g_pred1 / g_pred2 [rows,C] = its gradients (sign(0) = 0, as torch).
+ * g_move1 [rows,C] (optional, must not alias the outputs): gradient other loss terms already left on pred1 -- the
+ * attentive entropy of main.py:559-562 reads the target logits of this pass; it is added to g_pred1 and then zeroed,
+ * so that the buffer it lives in can carry the other pass's gradient.                                            */
+int ta3n_mcd_loss_fwd_bwd(const float* pred1, const float* pred2, int rows, int C, const int* valid_rows, float* loss,
+                          float* g_pred1, float* g_pred2, float* g_move1, ta3n_stream_t stream);
+/* dst[i] += src[i] for n floats (both 16-byte aligned): sums the gradient buckets of two backward passes.          */
+int ta3n_accumulate(float* dst, const float* src, long long n, ta3n_stream_t stream);
 
 /* ---- the training step as one step program (SURVEY 8a rows a1-a13 + 8f row n1) ----------------------------- */
 /* main.py:418 (model forward, models.py:545-722 trn-m branch), main.py:446, 508-538, 559-562 (composed loss:

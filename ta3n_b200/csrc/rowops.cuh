@@ -721,6 +721,144 @@ __global__ void __launch_bounds__(1024) loss_reduce_kernel(const float* __restri
 __global__ void counter_inc_kernel(unsigned long long* ctr) {
   pdl_wait(); ctr[0] += 1ull; }
 
+// ---- loss terms of ens_DA='MCD' (main.py:446-448, 548-556; loss.py:29-30) ---------------------------
+// One block: warp w takes rows w, w + 8, ...; every row's term is added to its warp's running sum in row order and
+// the eight warp sums are added in warp order, so the scalar is the same bit pattern on every replay.
+constexpr int kMcdThreads = 256;
+
+__device__ __forceinline__ float row_max(const float* p, int C, int lane) {
+  float mx = -INFINITY;
+  for (int c = lane; c < C; c += 32) mx = fmaxf(mx, p[c]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  return mx;
+}
+
+__device__ __forceinline__ void block_add_scalar(float warp_total, float scale, float* out) {
+  __shared__ float red[kMcdThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) red[warp] = warp_total;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < kMcdThreads / 32; ++w) t += red[w];
+    out[0] += t * scale;
+  }
+}
+
+// loss += mean over the real rows r < valid_rows[0] of CE(pred[r], labels[r]);  g_pred = its gradient (0 on padding)
+__global__ void __launch_bounds__(kMcdThreads)
+ce_loss_kernel(const float* __restrict__ pred, const long long* __restrict__ labels, int rows, int C,
+               const int* __restrict__ valid_rows, float* __restrict__ loss, float* __restrict__ g_pred) {
+  pdl_wait();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int vs = valid_rows ? max(0, min(valid_rows[0], rows)) : rows;
+  const float inv = 1.f / (float)max(vs, 1);
+  float acc = 0.f;   // lane 0: this warp's sum of -log q_y
+  for (int r = warp; r < rows; r += kMcdThreads / 32) {
+    float* g = g_pred + (size_t)r * C;
+    if (r >= vs) {
+      for (int c = lane; c < C; c += 32) g[c] = 0.f;
+      continue;
+    }
+    const float* p = pred + (size_t)r * C;
+    const float mx = row_max(p, C, lane);
+    float se = 0.f;
+    for (int c = lane; c < C; c += 32) se += expf(p[c] - mx);
+    const float lse = logf(warp_sum(se));
+    const int y = (int)labels[r];
+    float ly = 0.f;
+    for (int c = lane; c < C; c += 32) {
+      const float lq = p[c] - mx - lse;
+      g[c] = (expf(lq) - (c == y ? 1.f : 0.f)) * inv;
+      if (c == y) ly = lq;
+    }
+    ly = warp_sum(ly);   // exactly one lane held log q_y
+    if (lane == 0) acc -= ly;
+  }
+  block_add_scalar(acc, inv, loss);
+}
+
+// Discrepancy of the two classifiers on the real rows r < valid_rows[1] (main.py:548-556):
+//   loss += -1/(n C) sum_r sum_c |s1_rc - s2_rc|,  s = softmax over C
+//   u_c = dloss/ds1_c = -sign(s1_c - s2_c) / (n C)   (sign(0) = 0, as torch's abs backward)
+//   g1_j = s1_j (u_j - sum_c s1_c u_c),  g2_j = s2_j (-u_j + sum_c s2_c u_c)
+// g_move1 (optional): gradient other loss terms left on pred1; it is added to g1 and cleared.
+__global__ void __launch_bounds__(kMcdThreads)
+mcd_loss_kernel(const float* __restrict__ p1, const float* __restrict__ p2, int rows, int C,
+                const int* __restrict__ valid_rows, float* __restrict__ loss, float* __restrict__ g1,
+                float* __restrict__ g2, float* __restrict__ g_move1) {
+  pdl_wait();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int vt = valid_rows ? max(0, min(valid_rows[1], rows)) : rows;
+  const float inv = 1.f / ((float)max(vt, 1) * (float)C);
+  float acc = 0.f;   // lane 0: this warp's sum of |s1 - s2|
+  for (int r = warp; r < rows; r += kMcdThreads / 32) {
+    const size_t o = (size_t)r * C;
+    if (r >= vt) {
+      for (int c = lane; c < C; c += 32) {
+        g1[o + c] = g_move1 ? g_move1[o + c] : 0.f;
+        g2[o + c] = 0.f;
+        if (g_move1) g_move1[o + c] = 0.f;
+      }
+      continue;
+    }
+    const float m1 = row_max(p1 + o, C, lane), m2 = row_max(p2 + o, C, lane);
+    float e1 = 0.f, e2 = 0.f;
+    for (int c = lane; c < C; c += 32) {
+      e1 += expf(p1[o + c] - m1);
+      e2 += expf(p2[o + c] - m2);
+    }
+    const float l1 = logf(warp_sum(e1)), l2 = logf(warp_sum(e2));
+    float sabs = 0.f, su1 = 0.f, su2 = 0.f;
+    for (int c = lane; c < C; c += 32) {
+      const float s1 = expf(p1[o + c] - m1 - l1), s2 = expf(p2[o + c] - m2 - l2);
+      const float d = s1 - s2;
+      const float u = d > 0.f ? -inv : (d < 0.f ? inv : 0.f);
+      sabs += fabsf(d);
+      su1 += s1 * u;
+      su2 += s2 * u;
+    }
+    sabs = warp_sum(sabs);
+    su1 = warp_sum(su1);
+    su2 = warp_sum(su2);
+    for (int c = lane; c < C; c += 32) {
+      const float s1 = expf(p1[o + c] - m1 - l1), s2 = expf(p2[o + c] - m2 - l2);
+      const float d = s1 - s2;
+      const float u = d > 0.f ? -inv : (d < 0.f ? inv : 0.f);
+      float a = s1 * (u - su1);
+      if (g_move1) {
+        a += g_move1[o + c];
+        g_move1[o + c] = 0.f;
+      }
+      g1[o + c] = a;
+      g2[o + c] = s2 * (su2 - u);
+    }
+    if (lane == 0) acc += sabs;
+  }
+  block_add_scalar(acc, -inv, loss);
+}
+
+// dst += src (n floats)
+__global__ void __launch_bounds__(256) accumulate_kernel(float* __restrict__ dst, const float* __restrict__ src,
+                                                         size_t n) {
+  pdl_wait();
+  const size_t n4 = n / 4;
+  float4* d4 = reinterpret_cast<float4*>(dst);
+  const float4* s4 = reinterpret_cast<const float4*>(src);
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n4; e += (size_t)gridDim.x * blockDim.x) {
+    float4 a = d4[e];
+    const float4 b = s4[e];
+    a.x += b.x;
+    a.y += b.y;
+    a.z += b.z;
+    a.w += b.w;
+    d4[e] = a;
+  }
+  for (size_t e = 4 * n4 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x)
+    dst[e] += src[e];
+}
+
 // ---- deterministic (weighted) column sums: bias gradients and the skinny head weight gradients ----
 //   out[k*ldo + n] = sum_seg sum_r  P_seg[r*ldp + k] * X_seg[r*ld + n]      k < N2 <= 32, n < N
 // P == nullptr -> N2 = 1 with unit weights (a plain column sum = a bias gradient).  The N2 x N outputs of

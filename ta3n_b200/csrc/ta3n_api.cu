@@ -876,13 +876,14 @@ int ta3n_video_head_bwd(const float* dropped, int M, int H, int C, const float* 
     TA3N_CUDA(cudaMemsetAsync(dbc, 0, sizeof(float) * C, st));
   }
   if (M == 0) return TA3N_OK;
-  TA3N_REQUIRE(dropped && Wc && d_feat_video, "null pointer");
-  const DropArgs d = make_drop(drop);
-  pre_launch("video_head_bwd", st);
-  launch_kernel(video_head_bwd_kernel, blocks_for((size_t)M * H, 256), 256, 0, st, g_pred, C, Wc, d_dropped_extra,
-                                                                         g_feat_video_ext, grad_scale, d,
-                                                                         d_feat_video, M, H);
-  TA3N_TRY(after_launch());
+  TA3N_REQUIRE(dropped && Wc, "null pointer");
+  if (d_feat_video) {
+    const DropArgs d = make_drop(drop);
+    pre_launch("video_head_bwd", st);
+    launch_kernel(video_head_bwd_kernel, blocks_for((size_t)M * H, 256), 256, 0, st, g_pred, C, Wc, d_dropped_extra,
+                  g_feat_video_ext, grad_scale, d, d_feat_video, M, H);
+    TA3N_TRY(after_launch());
+  }
   if (g_pred) {
     Arena arena(workspace, workspace_bytes);
     if (C <= 32) {   // dWc [C,H] = g_pred^T dropped: skinny -> weighted column sum
@@ -940,6 +941,41 @@ int ta3n_counter_inc(uint64_t* counter, ta3n_stream_t stream) {
   TA3N_REQUIRE(counter != nullptr, "null counter");
   pre_launch("counter_inc", S(stream));
   launch_kernel(counter_inc_kernel, 1, 1, 0, S(stream), reinterpret_cast<unsigned long long*>(counter));
+  return after_launch();
+}
+
+// ------------------------------------------------------------------------------------------------
+// ens_DA='MCD' loss terms (main.py:446-448, 548-556; loss.py:29-30)
+// ------------------------------------------------------------------------------------------------
+int ta3n_ce_loss_fwd_bwd(const float* pred, const long long* labels, int rows, int C, const int* valid_rows,
+                         float* loss, float* g_pred, ta3n_stream_t stream) {
+  TA3N_REQUIRE(rows >= 0 && C >= 1, "bad sizes");
+  if (rows == 0) return TA3N_OK;
+  TA3N_REQUIRE(pred && labels && loss && g_pred, "null pointer");
+  pre_launch("ce_loss", S(stream));
+  launch_kernel(ce_loss_kernel, 1, kMcdThreads, 0, S(stream), pred, labels, rows, C, valid_rows, loss, g_pred);
+  return after_launch();
+}
+
+int ta3n_mcd_loss_fwd_bwd(const float* pred1, const float* pred2, int rows, int C, const int* valid_rows, float* loss,
+                          float* g_pred1, float* g_pred2, float* g_move1, ta3n_stream_t stream) {
+  TA3N_REQUIRE(rows >= 0 && C >= 1, "bad sizes");
+  if (rows == 0) return TA3N_OK;
+  TA3N_REQUIRE(pred1 && pred2 && loss && g_pred1 && g_pred2, "null pointer");
+  TA3N_REQUIRE(g_pred1 != g_pred2 && g_move1 != g_pred1 && g_move1 != g_pred2, "gradient buffers must not alias");
+  pre_launch("mcd_loss", S(stream));
+  launch_kernel(mcd_loss_kernel, 1, kMcdThreads, 0, S(stream), pred1, pred2, rows, C, valid_rows, loss, g_pred1,
+                g_pred2, g_move1);
+  return after_launch();
+}
+
+int ta3n_accumulate(float* dst, const float* src, long long n, ta3n_stream_t stream) {
+  TA3N_REQUIRE(n >= 0, "bad size");
+  if (n == 0) return TA3N_OK;
+  TA3N_REQUIRE(dst && src, "null pointer");
+  TA3N_REQUIRE(aligned16(dst) && aligned16(src), "buffers must be 16-byte aligned");
+  pre_launch("accumulate", S(stream));
+  launch_kernel(accumulate_kernel, blocks_for((size_t)(n + 3) / 4, 256), 256, 0, S(stream), dst, src, (size_t)n);
   return after_launch();
 }
 

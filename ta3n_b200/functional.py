@@ -186,6 +186,10 @@ class PathSpec:
     use_attn_frame: bool = False
     drop_i: DropSpec = field(default_factory=DropSpec)
     drop_v: DropSpec = field(default_factory=DropSpec)
+    # the classification pass of ens_DA='MCD' (main.py:548-556): only the class logits feed its loss, so the video
+    # discriminator is not run, nor the frame discriminator unless the frame attention reads it; with reverse and
+    # mu == 0 nothing flows below the classifier (GRL_mu), so the backward stops at its weight gradient
+    classify_only: bool = False
 
 
 # parameter order expected by _VideoPathFunction (R = T-1):
@@ -258,12 +262,15 @@ def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: boo
     check(lib.ta3n_shared_fc_fwd(_p(xs), Bs * T, _p(xt), Bt * T, D, _p(w_sh), _p(b_sh), F, _dref(d_i),
                                  _p(feat), st))
     # 2. frame-level discriminator  (models.py:606-610)
-    hid_f, pred_frame = new("hid_f", M * T, F), new("pred_frame", M * T, 2)
-    batched = batch_gemms and not spec.use_attn_frame
+    frame_disc = not spec.classify_only or spec.use_attn_frame
+    hid_f = pred_frame = None
+    batched = batch_gemms and not spec.use_attn_frame and frame_disc
     if batched:
         check(lib.ta3n_fwd_batch_begin())
-    check(lib.ta3n_disc_fwd(_p(feat), M * T, F, F, _p(w1f), _p(b1f), _p(w2f), _p(b2f), _p(hid_f),
-                            _p(pred_frame), st))
+    if frame_disc:
+        hid_f, pred_frame = new("hid_f", M * T, F), new("pred_frame", M * T, 2)
+        check(lib.ta3n_disc_fwd(_p(feat), M * T, F, F, _p(w1f), _p(b1f), _p(w2f), _p(b2f), _p(hid_f),
+                                _p(pred_frame), st))
     # 2b. frame attention  (models.py:612-614)
     if spec.use_attn_frame:
         feat_in = new("feat_in", M * T, F)
@@ -297,16 +304,18 @@ def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: boo
     check(lib.ta3n_video_head_fwd(_p(feat_video), M, H, Cn, _p(w_c), _p(b_c), _dref(d_v), _p(dropped),
                                   _p(pred_video), st))
     # 6. video-level discriminator  (models.py:694-698)
-    hid_v, pred_dom_video = new("hid_v", M, H), new("pred_dom_video", M, 2)
-    check(lib.ta3n_disc_fwd(_p(dropped), M, H, H, _p(w1v), _p(b1v), _p(w2v), _p(b2v), _p(hid_v),
-                            _p(pred_dom_video), st))
+    hid_v = pred_dom_video = None
+    if not spec.classify_only:
+        hid_v, pred_dom_video = new("hid_v", M, H), new("pred_dom_video", M, 2)
+        check(lib.ta3n_disc_fwd(_p(dropped), M, H, H, _p(w1v), _p(b1v), _p(w2v), _p(b2v), _p(hid_v),
+                                _p(pred_dom_video), st))
 
     saved = dict(feat=feat, hid_f=hid_f, pred_frame=pred_frame, feat_in=feat_in, act=act, feat_rel=feat_rel,
                  hid_r=hid_r, pred_rel=pred_rel, attn=attn, dropped=dropped, hid_v=hid_v)
     if hid_a is not None:
         saved["hid_a"] = hid_a
-    outputs = (feat.view(M, T, F), pred_frame.view(M, T, 2), attn, pred_rel, feat_video, pred_video,
-               pred_dom_video, dropped)
+    outputs = (feat.view(M, T, F), None if pred_frame is None else pred_frame.view(M, T, 2), attn, pred_rel,
+               feat_video, pred_video, pred_dom_video, dropped)
     return saved, outputs, (Bs, Bt, D, T, F, H, Cn)
 
 
@@ -321,7 +330,7 @@ def path_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, bufs: 
     and on forward activations, so it runs on that stream concurrently with the video -> relation chain and
     WRITES d_feat; the TRN dgrad then accumulates into it."""
     stage_done = stage_done or (lambda name: None)
-    frame_parallel = side_stream is not None and not spec.use_attn_frame
+    frame_parallel = side_stream is not None and not spec.use_attn_frame and not spec.classify_only
     lib = _lib.load()
     st = _stream()
     Bs, Bt, D, T, F, H, Cn = dims
@@ -359,22 +368,29 @@ def path_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, bufs: 
         frame_done.record(side_stream)
 
     # 6'. video discriminator: d_dropped = -beta1 * dgrad  (+ what other consumers of `dropped` sent back: the second
-    #     classifier of MCD, models.py:716-720 -- it sits behind GRL_mu like the first one, so its gradient joins here)
+    #     classifier of MCD, models.py:716-720 -- it sits behind GRL_mu like the first one, so its gradient joins here;
+    #     a caller that wrote it straight into this step's "d_dropped" buffer saves the copy)
     d_dropped = new("d_dropped", M, H)
     g_dropped = g("dropped")
-    if g_dropped is not None:
+    if g_dropped is not None and g_dropped.data_ptr() != d_dropped.data_ptr():
         d_dropped.copy_(g_dropped.reshape(M, H))
-    ws = wsp("disc_v", lib.ta3n_disc_bwd_workspace_bytes(M, H, H))
-    check(lib.ta3n_disc_bwd(_p(dropped), M, H, H, _p(w1v), _p(w2v), _p(hid_v), _p(g("pred_dom_video")),
-                            float(spec.beta[1]), _p(d_dropped), 1 if g_dropped is not None else 0, _p(dw1v), _p(db1v),
-                            _p(dw2v), _p(db2v), _p(ws), ws.numel(), st))
+    if not spec.classify_only:
+        ws = wsp("disc_v", lib.ta3n_disc_bwd_workspace_bytes(M, H, H))
+        check(lib.ta3n_disc_bwd(_p(dropped), M, H, H, _p(w1v), _p(w2v), _p(hid_v), _p(g("pred_dom_video")),
+                                float(spec.beta[1]), _p(d_dropped), 1 if g_dropped is not None else 0, _p(dw1v),
+                                _p(db1v), _p(dw2v), _p(db2v), _p(ws), ws.numel(), st))
+    elif g_dropped is None:
+        d_dropped = None
     # 5'. classifier + dropout_v (+ optional GRL_mu around both heads, models.py:682-684)
-    G = new("G", M, H)
+    cut = spec.classify_only and spec.reverse and spec.mu == 0.0     # GRL_mu passes nothing further down
+    G = None if cut else new("G", M, H)
     ws = wsp("vhead", lib.ta3n_video_head_bwd_workspace_bytes(M, H, Cn))
     check(lib.ta3n_video_head_bwd(_p(dropped), M, H, Cn, _p(w_c), _dref(d_v), _p(g("pred_video")), _p(d_dropped),
                                   _p(g("feat_video")), float(-spec.mu) if spec.reverse else 1.0, _p(G),
                                   _p(dw_c), _p(db_c), _p(ws), ws.numel(), st))
     stage_done("video")
+    if cut:
+        return
     # 4'. relation discriminators / attention (attention weights are NOT detached, SURVEY 3.3)
     d_feat_rel = new("d_feat_rel", M, R, H)
     ws = wsp("relattn", lib.ta3n_relattn_bwd_workspace_bytes(M, R, H))
@@ -413,7 +429,7 @@ def path_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, bufs: 
         g_pf = acc
         check(lib.ta3n_frame_attn_bwd(_p(feat), _p(pred_frame), M * T, F, _p(d_feat), _p(g_pf), st))
     # 2'. frame discriminator: d_feat += -beta2 * dgrad   (unless it already ran as the parallel branch)
-    if not frame_parallel:
+    if not frame_parallel and (not spec.classify_only or spec.use_attn_frame):
         frame_disc_bwd(st, 1)
     stage_done("frame")
     # 1'. shared layer (wgrad only; the input features carry no gradient)

@@ -37,6 +37,7 @@ from ._lib import check
 _P = TF._p
 _N_LATE = 6     # path_parameters()[0:6] = shared layer W,b + frame discriminator W1,b1,W2,b2: produced last
 _ALIGN = 64     # floats: every tensor of a flat buffer starts 256-byte aligned (vector stores, TMA operands)
+_PASS2_KEY = 0x6A09E667F3BCC908     # seed of MCD's second pass = step seed ^ this (its masks differ from pass 1's)
 
 
 @dataclass
@@ -60,6 +61,16 @@ def beta_dann(p: float) -> float:
     return 2.0 / (1.0 + math.exp(-10.0 * p)) - 1.0
 
 
+def step_parameters(model):
+    """The tensors of the step's flat buffers: ``path_parameters()`` and, under ens_DA='MCD', the second classifier
+    (models.py:276-279) appended, so that it lands in the early part of the bucket next to the video head."""
+    params = model.path_parameters()
+    if getattr(model, "ens_DA", "none") == "MCD":
+        head2 = model.fc_classifier_video_source_2
+        params = params + [head2.weight, head2.bias]
+    return params
+
+
 def bucket_layout(params):
     """Order and offsets (in floats) of the path's tensors inside a flat buffer: the order in which the
     backward finishes their gradients, [video head, video disc, relation discs, TRN | frame disc, shared layer],
@@ -78,7 +89,7 @@ def flatten_parameters(model) -> torch.Tensor:
     """Re-point the ``.data`` of the path's parameters at views of ONE flat fp32 buffer (bucket_layout order), so
     that the optimizer is a single pass over contiguous memory.  Values are preserved; idempotent.  The
     Parameter objects (and hence state_dict / load_state_dict / checkpoints) are unchanged."""
-    params = model.path_parameters()
+    params = step_parameters(model)
     order, offs, total, _ = bucket_layout(params)
     flat = getattr(model, "_ta3n_flat_params", None)
     if (flat is not None and flat.numel() == total and flat.device == params[0].device and
@@ -108,7 +119,7 @@ class TrainStep:
                  overlap_allreduce: Optional[bool] = None, graph_collectives: Optional[bool] = None,
                  optimizer: Optional[SGDNesterov] = None, mode: Optional[str] = None,
                  class_weight: Optional[torch.Tensor] = None, domain_weight: Sequence[float] = (1.0, 1.0),
-                 allreduce: Optional[str] = None):
+                 allreduce: Optional[str] = None, mu: float = 0.0):
         """mode: 'legacy' (default) = the per-operator sequence (25 launches in one CUDA graph; the only mode that
         supports use_attn_frame); 'phased' = the step program as 14 launches (ta3n_step_run_phased; default when class /
         domain weights or a scheduled beta are given).  class_weight / domain_weight: the weights of criterion /
@@ -117,17 +128,41 @@ class TrainStep:
         allreduce (world > 1): 'peer' = this library's one-kernel all-reduce over NVLink peer / NVSwitch multicast
         memory (csrc/allreduce.cuh; the gradient bucket then lives in symmetric memory and the whole iteration --
         step, all-reduce, optimizer -- is one CUDA graph), 'nccl' = torch.distributed all_reduce between graphs;
-        default: 'peer' when symmetric memory can be set up (and no NCCL overlap option was asked for), else 'nccl'."""
+        default: 'peer' when symmetric memory can be set up (and no NCCL overlap option was asked for), else 'nccl'.
+
+        ens_DA='MCD' (mode 'legacy' only): the iteration of main.py:418-583 with --ens_DA MCD is two passes, both in
+        the one graph.  Pass 1 (reverse=False) is the step above plus the second classifier on the source rows and its
+        class CE (main.py:447-448).  Pass 2 (reverse=True) runs the target rows only, with their own dropout masks
+        (pass2_seeds), for -dis_MCD(out_t, out_t_2) (main.py:548-556, loss.py:29-30); its target logits of the first
+        classifier are also those the attentive entropy reads (main.py:559-562 runs after the second forward).  Its
+        gradient reaches the classifiers directly and everything below the video feature scaled by -mu (GRL_mu,
+        models.py:682-684); with mu == 0 its backward stops at the classifiers.  The two passes' gradients are summed
+        before the all-reduce, clipping and SGD.  dis_MCD averages over the real target rows of the batch; a batch
+        with no real target row contributes 0 (the reference would take the mean of an empty tensor).
+        mu: the GRL coefficient of pass 2 (--mu, fixed at capture); non-zero only under MCD."""
         if not model.training:
             raise ValueError("TrainStep needs model.train() (dropout state is fixed at construction)")
-        if model.use_attn == "general" or getattr(model, "ens_DA", "none") != "none" or \
-                model.frame_aggregation != "trn-m":
+        ens = getattr(model, "ens_DA", "none")
+        if model.use_attn == "general" or ens not in ("none", "MCD") or model.frame_aggregation != "trn-m":
             # the off-path variants (SURVEY 8f n4) run through VideoModel.forward + autograd; the captured step covers
-            # the shipped configurations (use_attn 'TransAttn' / 'none', one classifier)
+            # the shipped configurations (use_attn 'TransAttn' / 'none') and MCD's two-pass iteration
             raise NotImplementedError("TrainStep covers frame_aggregation='trn-m', use_attn in ('TransAttn', 'none') and "
-                                      "ens_DA='none'; train the other variants with model(...) + loss.backward()")
+                                      "ens_DA in ('none', 'MCD'); train the other variants with model(...) + "
+                                      "loss.backward()")
+        self.mcd = ens == "MCD"
+        self.mu = float(mu)
+        if self.mu != 0.0 and not self.mcd:
+            raise ValueError("mu scales the gradient of MCD's reverse pass (ens_DA='MCD'); without MCD it does nothing")
+        if self.mcd:
+            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
+                raise NotImplementedError("ens_DA='MCD' runs in mode='legacy' only (the step program has one pass)")
+            if class_weight is not None or any(float(b) < 0 for b in beta) or \
+                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
+                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
+                                          "(mode='phased'), which does not cover ens_DA='MCD'")
+            mode = "legacy"
         self.model = model
-        self.params = model.path_parameters()
+        self.params = step_parameters(model)
         dev = self.params[0].device
         if dev.type != "cuda":
             raise _lib.Ta3nError("TrainStep needs the model on a CUDA device; there is no CPU path")
@@ -176,8 +211,10 @@ class TrainStep:
             raise ValueError("class_weight needs mode='phased'")
         self._overlap_requested = bool(overlap_allreduce)
         self.split = (self.world > 1) if overlap_allreduce is None else bool(overlap_allreduce)
-        if model.use_attn_frame != "none" or mode != "legacy":
-            self.split = False     # frame attention couples the TRN and frame-discriminator gradients
+        if model.use_attn_frame != "none" or mode != "legacy" or self.mcd:
+            # frame attention couples the TRN and frame-discriminator gradients; MCD's second pass adds to the early
+            # bucket after the first pass has finished it
+            self.split = False
         # graph_collectives=True captures the two NCCL all-reduces INSIDE the step's graph.  It works and is
         # marginally faster (N=2: 0.371 vs 0.378 ms/step) but process-group teardown then hangs while the graphs
         # are alive (observed on torch 2.11 / NCCL 2.28), so it is opt-in; the default is two graphs with the
@@ -219,7 +256,8 @@ class TrainStep:
             if not (self.flags & 1) and model.use_attn == "none":
                 idle += list(range(6 + 2 * R, 6 + 6 * R))             # relation discriminators
             if not (self.flags & 2) and not (self.flags & 8):
-                idle += list(range(len(self.params) - 4, len(self.params)))     # video discriminator
+                n_core = 6 + 6 * R + 6
+                idle += list(range(n_core - 4, n_core))                         # video discriminator
             self.active_mask = None
             if idle:
                 self.active_mask = torch.ones_like(self.flat_grad)
@@ -266,13 +304,15 @@ class TrainStep:
             use_attn=model.use_attn != "none", use_attn_frame=model.use_attn_frame != "none",
             drop_i=TF.DropSpec(p=di, seed=seed, step=self.step_counter) if di > 0 else TF.DropSpec(),
             drop_v=TF.DropSpec(p=dv, seed=seed ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec())
+        if self.mcd:
+            self._init_mcd(seed, di, dv, offs)
         self.outputs = None
         self.branch_stream = torch.cuda.Stream(device=dev) if parallel_branches else None
         self.overlap_wgrad = bool(overlap_wgrad)
         self.side_stream = torch.cuda.Stream(device=dev) if self.overlap_wgrad else None
         # reducing the early bucket on a forked stream was slower than one all-reduce behind the step -- the collective is
         # latency / rank-skew bound (a second kernel pays the fixed cost again and competes for SMs), so the split is opt-in
-        self.early_ar = os.environ.get("TA3N_EARLY_ALLREDUCE", "0") == "1"
+        self.early_ar = os.environ.get("TA3N_EARLY_ALLREDUCE", "0") == "1" and not self.mcd
         self.ar_stream = torch.cuda.Stream(device=dev) if (self.overlap_wgrad and self.ar is not None) else None
         self.launches_per_step = 0               # kernels of libta3n_sm90.so per step (counted at capture)
         self.use_graph = bool(use_graph)
@@ -288,6 +328,70 @@ class TrainStep:
                 self.graphs[slot] = self._capture()
             self.active = 0
             self.xs, self.xt, self.labels, self.valid = self.slots[0]
+
+    def _init_mcd(self, seed, di, dv, offs):
+        """State of MCD's second pass: its dropout seeds, buffers, and a second gradient bucket with the bucket's
+        layout.  Pass 2 writes its parameter gradients there (every backward entry writes, none accumulates) and one
+        elementwise add folds the slots it reached into the bucket: with mu == 0 the two classifiers, which the
+        early part of the bucket ends with; otherwise the whole bucket (the video-discriminator slots, and the frame
+        discriminator's without frame attention, stay zero)."""
+        dev, f32 = self.device, dict(device=self.device, dtype=torch.float32)
+        M, Bs, Bt, C, H = self.M, self.Bs, self.Bt, self.C, self.model.fc_classifier_video_source.weight.shape[1]
+        s2 = (seed ^ _PASS2_KEY) & (2 ** 63 - 1)
+        self.pass2_seeds = (s2, s2 ^ 0x9E3779B9)       # (drop_i, drop_v) of pass 2, keyed by the same step counter
+        self.spec2 = TF.PathSpec(
+            num_segments=self.T, beta=self.spec.beta, mu=self.mu, reverse=True, use_attn=self.spec.use_attn,
+            use_attn_frame=self.spec.use_attn_frame, classify_only=True,
+            drop_i=TF.DropSpec(p=di, seed=s2, step=self.step_counter) if di > 0 else TF.DropSpec(),
+            drop_v=TF.DropSpec(p=dv, seed=s2 ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec())
+        self.bufs2 = TF.Buffers(dev, persistent=True)
+        self.x_none = torch.zeros(0, self.T, self.D, **f32)            # pass 2 has no source half
+        # pass 2 writes its first classifier's logits over the target rows of pass 1's: those rows of pass 1 feed no
+        # loss, and the attentive entropy (loss kernel of pass 1) reads the target logits of pass 2
+        pred_video = self.bufs.get("pred_video", M, C)
+        self.bufs2.pool["pred_video"] = pred_video[Bs:]
+        self.pred2_s, self.pred2_t = torch.zeros(Bs, C, **f32), torch.zeros(Bt, C, **f32)
+        self.head2_scratch = torch.zeros(max(Bs, Bt), H, **f32)       # the head operator's (unused) dropped copy
+        self.g_video2 = torch.zeros(M, C, **f32)     # CE(out_s_2) gradient; target rows stay 0 (pass 1 has no target term)
+        self.g_video_t, self.g_video2_t = torch.zeros(Bt, C, **f32), torch.zeros(Bt, C, **f32)
+        self.flat_grad2 = torch.zeros_like(self.flat_grad)
+        self.grad_views2 = [self.flat_grad2[offs[i]:offs[i] + p.numel()].view_as(p) for i, p in enumerate(self.params)]
+        cls = len(self.params) - 8                   # fc_classifier_video_source.weight (then bias, video disc, head 2)
+        self.acc_range = (offs[cls], self.early_numel) if self.mu == 0.0 else (0, self.flat_grad.numel())
+
+    def _enqueue_mcd_pass2_forward(self, lib, st):
+        """Pass 2's forward (target rows only, fresh masks) and its second classifier."""
+        saved2, out2, dims2 = TF.path_forward(self.spec2, self.x_none, self.xt, self.params, self.bufs2,
+                                              batch_gemms=True)
+        w2, b2 = self.params[-2], self.params[-1]
+        check(lib.ta3n_video_head_fwd(_P(saved2["dropped"]), self.Bt, w2.shape[1], self.C, _P(w2), _P(b2), None,
+                                      _P(self.head2_scratch), _P(self.pred2_t), st))
+        self.outputs2 = out2
+        return saved2, dims2
+
+    def _enqueue_head2_bwd(self, lib, st, bufs, dropped, rows, g_pred, d_dropped, gviews):
+        w2 = self.params[-2]
+        H = w2.shape[1]
+        ws = bufs.workspace("vhead2", lib.ta3n_video_head_bwd_workspace_bytes(rows, H, self.C))
+        check(lib.ta3n_video_head_bwd(_P(dropped), rows, H, self.C, _P(w2), None, _P(g_pred), None, None, 1.0,
+                                      _P(d_dropped), _P(gviews[-2]), _P(gviews[-1]), _P(ws), ws.numel(), st))
+
+    def _enqueue_mcd_pass2_backward(self, lib, st, saved2, dims2):
+        """Pass 2's backward into the second bucket, then bucket += the slots it reached."""
+        cut = self.mu == 0.0
+        d_dropped = None if cut else self.bufs2.get("d_dropped", self.Bt, self.params[-2].shape[1])
+        check(lib.ta3n_wgrad_defer_begin())
+        self._enqueue_head2_bwd(lib, st, self.bufs2, saved2["dropped"], self.Bt, self.g_video2_t, d_dropped,
+                                self.grad_views2)
+        gin = {"pred_video": self.g_video_t}
+        if d_dropped is not None:
+            gin["dropped"] = d_dropped
+        TF.path_backward(self.spec2, dims2, self.x_none, self.xt, self.params, saved2, gin, self.grad_views2,
+                         self.bufs2)
+        ws = self.bufs2.workspace("wgrad", lib.ta3n_wgrad_defer_workspace_bytes())
+        check(lib.ta3n_wgrad_defer_flush(_P(ws), ws.numel(), st))
+        lo, hi = self.acc_range
+        check(lib.ta3n_accumulate(_P(self.flat_grad[lo:]), _P(self.flat_grad2[lo:]), hi - lo, st))
 
     # -- gradient bucket / all-reduce ------------------------------------------------------------------
     def _alloc_gradient_bucket(self, n, allreduce):
@@ -478,10 +582,23 @@ class TrainStep:
         saved, outputs, dims = TF.path_forward(self.spec, self.xs, self.xt, self.params, self.bufs, batch_gemms=True)
         self.outputs = outputs
         _, pred_frame, _, pred_rel, _, pred_video, pred_dom, _ = outputs
+        if self.mcd:
+            # second classifier on the source rows (its target logits of this pass feed no loss), then pass 2's forward
+            w2, b2 = self.params[-2], self.params[-1]
+            check(lib.ta3n_video_head_fwd(_P(saved["dropped"]), self.Bs, w2.shape[1], self.C, _P(w2), _P(b2), None,
+                                          _P(self.head2_scratch), _P(self.pred2_s), st))
+            saved2, dims2 = self._enqueue_mcd_pass2_forward(lib, st)
         check(lib.ta3n_loss_fwd_bwd(_P(pred_video), _P(self.labels), _P(pred_rel), _P(pred_dom), _P(pred_frame),
                                     self.Bs, self.Bt, self.T, self.R, self.C, self.gamma, self.flags,
                                     _P(self.valid), _P(self.loss), _P(self.g_video), _P(self.g_rel), _P(self.g_dom),
                                     _P(self.g_frame), _P(self.loss_ws), self.loss_ws.numel(), st))
+        if self.mcd:
+            check(lib.ta3n_ce_loss_fwd_bwd(_P(self.pred2_s), _P(self.labels), self.Bs, self.C, _P(self.valid),
+                                           _P(self.loss), _P(self.g_video2), st))
+            # the attentive entropy's gradient on the target rows belongs to pass 2's logits: moved out of g_video
+            check(lib.ta3n_mcd_loss_fwd_bwd(_P(pred_video[self.Bs:]), _P(self.pred2_t), self.Bt, self.C, _P(self.valid),
+                                            _P(self.loss), _P(self.g_video_t), _P(self.g_video2_t),
+                                            _P(self.g_video[self.Bs:]), st))
         gin = {"pred_video": self.g_video, "pred_rel": self.g_rel, "pred_dom_video": self.g_dom,
                "pred_frame": self.g_frame}
         # The data-gradient chain runs first; the weight-gradient GEMMs / bias sums it leaves behind are deferred
@@ -524,10 +641,18 @@ class TrainStep:
                 check(lib.ta3n_wgrad_defer_begin())
 
         check(lib.ta3n_wgrad_defer_begin())
+        if self.mcd:
+            # CE(out_s_2)'s data gradient joins the video discriminator's on `dropped`, written in place
+            d_dropped = self.bufs.get("d_dropped", self.M, self.params[-2].shape[1])
+            self._enqueue_head2_bwd(lib, st, self.bufs, saved["dropped"], self.M, self.g_video2, d_dropped,
+                                    self.grad_views)
+            gin["dropped"] = d_dropped
         TF.path_backward(self.spec, dims, self.xs, self.xt, self.params, saved, gin, self.grad_views, self.bufs,
                          stage_done=stage_done, side_stream=self.branch_stream)
         if self.overlap_wgrad:
             main.wait_stream(side)            # join
+        if self.mcd:
+            self._enqueue_mcd_pass2_backward(lib, st, saved2, dims2)
         if early_ar:
             main.wait_stream(self.ar_stream)
             self._enqueue_allreduce(self.early_numel, None, slot=1)      # the late 38 %: the only exposed part
