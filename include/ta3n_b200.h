@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define TA3N_ABI_VERSION 4
+#define TA3N_ABI_VERSION 5
 
 enum {
   TA3N_OK = 0,
@@ -275,6 +275,22 @@ int ta3n_mcd_loss_fwd_bwd(const float* pred1, const float* pred2, int rows, int 
                           float* g_pred1, float* g_pred2, float* g_move1, ta3n_stream_t stream);
 /* dst[i] += src[i] for n floats (both 16-byte aligned): sums the gradient buckets of two backward passes.          */
 int ta3n_accumulate(float* dst, const float* src, long long n, ta3n_stream_t stream);
+
+/* ---- device-resident input pipeline (main.py:343-372 from feature banks in device memory) ---------------------- */
+/* One launch fills the input slot of a paired mini-batch for BOTH domains, for use as the first launch of a captured
+ * training step.  Per domain: bank [n_rows, row_floats] fp32 (16-byte aligned; row_floats % 4 == 0), the epoch's row
+ * list rows [n_epoch] int32 (bank row of every epoch position) and, source only, its label list labels [n_epoch]
+ * int64; the slot x [batch, row_floats] (16-byte aligned) and, source only, y [batch] int64.
+ * state [2] uint32: {iteration i, arrival counter (0 between launches)}.  The launch copies the rows of epoch
+ * positions [i*batch, min((i+1)*batch, n_epoch)) into the slot, zero-fills the rest (main.py:359-364 pads with zero
+ * dummies; padded labels are 0), writes valid_rows [2] = {real source rows, real target rows} (the pair
+ * ta3n_loss_fwd_bwd and the step program read) and advances state[0] by one; the last CTA to finish advances it, so
+ * there is no extra launch.  Offsets are 64-bit (banks above 2^31 floats are fine).  A bank row id outside
+ * [0, n_rows) gives a NaN row.  Kernel label "gather_batch".                                                        */
+int ta3n_gather_batch(const float* bank_s, long long n_rows_s, const int* rows_s, const long long* labels_s,
+                      long long n_epoch_s, int batch_s, float* x_s, long long* y_s,
+                      const float* bank_t, long long n_rows_t, const int* rows_t, long long n_epoch_t, int batch_t,
+                      float* x_t, long long row_floats, int* valid_rows, unsigned int* state, ta3n_stream_t stream);
 
 /* ---- the training step as one step program (SURVEY 8a rows a1-a13 + 8f row n1) ----------------------------- */
 /* main.py:418 (model forward, models.py:545-722 trn-m branch), main.py:446, 508-538, 559-562 (composed loss:

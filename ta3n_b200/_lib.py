@@ -11,7 +11,7 @@ import threading
 
 from . import build as _build
 
-ABI_VERSION = 4     # TA3N_ABI_VERSION of include/ta3n_b200.h that SIGNATURES mirrors
+ABI_VERSION = 5     # TA3N_ABI_VERSION of include/ta3n_b200.h that SIGNATURES mirrors
 
 TA3N_GEMM_FP32_SIMT = 0
 TA3N_GEMM_TF32_TCGEN05 = 1
@@ -105,6 +105,8 @@ SIGNATURES = {
     "ta3n_ce_loss_fwd_bwd": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP]),
     "ta3n_mcd_loss_fwd_bwd": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
     "ta3n_accumulate": (_I, [_VP, _VP, C.c_longlong, _VP]),
+    "ta3n_gather_batch": (_I, [_VP, C.c_longlong, _VP, _VP, C.c_longlong, _I, _VP, _VP,
+                               _VP, C.c_longlong, _VP, C.c_longlong, _I, _VP, C.c_longlong, _VP, _VP, _VP]),
     "ta3n_step_workspace_bytes": (_SZ, [C.POINTER(StepDesc)]),
     "ta3n_step_run_phased": (_I, [C.POINTER(StepDesc), _VP]),
     "ta3n_allreduce_flag_bytes": (_SZ, [_I]),

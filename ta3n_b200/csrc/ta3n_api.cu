@@ -8,6 +8,7 @@
 #include "optim.cuh"
 #include "step_plan.cuh"
 #include "allreduce.cuh"
+#include "gather.cuh"
 
 #include <functional>
 
@@ -976,6 +977,36 @@ int ta3n_accumulate(float* dst, const float* src, long long n, ta3n_stream_t str
   TA3N_REQUIRE(aligned16(dst) && aligned16(src), "buffers must be 16-byte aligned");
   pre_launch("accumulate", S(stream));
   launch_kernel(accumulate_kernel, blocks_for((size_t)(n + 3) / 4, 256), 256, 0, S(stream), dst, src, (size_t)n);
+  return after_launch();
+}
+
+// ------------------------------------------------------------------------------------------------
+// device-resident input pipeline (include/ta3n_b200.h: ta3n_gather_batch)
+// ------------------------------------------------------------------------------------------------
+int ta3n_gather_batch(const float* bank_s, long long n_rows_s, const int* rows_s, const long long* labels_s,
+                      long long n_epoch_s, int batch_s, float* x_s, long long* y_s,
+                      const float* bank_t, long long n_rows_t, const int* rows_t, long long n_epoch_t, int batch_t,
+                      float* x_t, long long row_floats, int* valid_rows, unsigned int* state, ta3n_stream_t stream) {
+  TA3N_REQUIRE(batch_s >= 1 && batch_t >= 1 && batch_s + batch_t <= 65535, "batch sizes must be >= 1, together <= 65535");
+  TA3N_REQUIRE(row_floats >= 4 && row_floats % 4 == 0, "row_floats must be a positive multiple of 4 (16-byte rows)");
+  TA3N_REQUIRE(n_epoch_s >= 1 && n_epoch_t >= 1, "empty epoch");
+  TA3N_REQUIRE(n_rows_s >= 1 && n_rows_t >= 1 && n_rows_s <= INT32_MAX && n_rows_t <= INT32_MAX,
+               "bank rows must be in [1, 2^31) (row lists are int32)");
+  TA3N_REQUIRE(n_rows_s <= INT64_MAX / row_floats && n_rows_t <= INT64_MAX / row_floats, "bank too large");
+  TA3N_REQUIRE(bank_s && rows_s && labels_s && x_s && y_s, "null source pointer");
+  TA3N_REQUIRE(bank_t && rows_t && x_t, "null target pointer");
+  TA3N_REQUIRE(valid_rows && state, "null valid_rows / state");
+  TA3N_REQUIRE(aligned16(bank_s) && aligned16(bank_t) && aligned16(x_s) && aligned16(x_t),
+               "banks and slots must be 16-byte aligned");
+  GatherDomain s{reinterpret_cast<const float4*>(bank_s), n_rows_s, rows_s, labels_s, n_epoch_s,
+                 reinterpret_cast<float4*>(x_s), y_s, batch_s};
+  GatherDomain t{reinterpret_cast<const float4*>(bank_t), n_rows_t, rows_t, nullptr, n_epoch_t,
+                 reinterpret_cast<float4*>(x_t), nullptr, batch_t};
+  const long long row_f4 = row_floats / 4;
+  const dim3 grid((unsigned)((row_f4 + kGatherChunk - 1) / kGatherChunk), (unsigned)(batch_s + batch_t));
+  TA3N_REQUIRE(grid.x <= 65535u, "rows too long");
+  pre_launch("gather_batch", S(stream));
+  launch_kernel(gather_batch_kernel, grid, kGatherThreads, 0, S(stream), s, t, row_f4, valid_rows, state);
   return after_launch();
 }
 

@@ -11,9 +11,11 @@ This module offers
   are gathered ONCE into a `(num_videos, T, feat_dim)` fp32 `.npy` shard that is memory-mapped afterwards;
 * `PairedFeatureLoader`: the `enumerate(zip(source_loader, target_loader))` of `main.py:343-346` with
   `RandomSampler` order, assembling every paired mini-batch directly into (pinned) staging buffers on a
-  background thread, ready for `TrainStep.prefetch()`.
+  background thread, ready for `TrainStep.prefetch()`;
+* `DeviceFeatureBank` + `DevicePairedSampler`: the same epochs with the shards resident in device memory; each
+  mini-batch is gathered by the first launch of the captured step (`TrainStep(..., sampler=...)`).
 
-Host-side code only: no device work happens here.
+Both paired paths draw their epochs from `paired_epoch_plan`, so that one seed gives the same batches on either.
 """
 from __future__ import annotations
 
@@ -230,6 +232,25 @@ class PackedTSNDataSet(data.Dataset):
         out_labels.numpy()[:k] = self.labels[indices]
 
 
+def paired_epoch_length(lengths: Sequence[int], batch_sizes: Sequence[int]) -> int:
+    """Iterations of one paired epoch: zip stops with the shorter loader, each ending with one short batch."""
+    return min(-(-int(n) // int(b)) for n, b in zip(lengths, batch_sizes))
+
+
+def paired_epoch_plan(gen: torch.Generator, lengths: Sequence[int],
+                      batch_sizes: Sequence[int]) -> Tuple[List[np.ndarray], int]:
+    """The sampling decision of one epoch of main.py:343-346 (RandomSampler per domain, main.py:188, 199): one
+    `torch.randperm` per dataset from `gen`, source first, and the epoch length.  Batch `it` of domain d is
+    `epoch_batch(perms[d], it, batch_sizes[d])`.  Returns (perms, n_iter)."""
+    perms = [torch.randperm(int(n), generator=gen).numpy() for n in lengths]
+    return perms, paired_epoch_length(lengths, batch_sizes)
+
+
+def epoch_batch(perm: np.ndarray, it: int, batch: int) -> np.ndarray:
+    """Dataset positions of batch `it` (the last one of an epoch may be short)."""
+    return perm[it * batch:(it + 1) * batch]
+
+
 class PairedFeatureLoader:
     """`enumerate(zip(source_loader, target_loader))` of main.py:343-346 for two `PackedTSNDataSet`s: each epoch
     visits both sets in an independent random permutation (RandomSampler, main.py:188, 199), stops with the
@@ -260,11 +281,10 @@ class PairedFeatureLoader:
             self.buffers.append(slot)
 
     def __len__(self):
-        return min(-(-len(ds) // b) for ds, b in zip(self.sets, self.batch))
+        return paired_epoch_length([len(ds) for ds in self.sets], self.batch)
 
     def __iter__(self) -> Iterator:
-        perms = [torch.randperm(len(ds), generator=self.gen).numpy() for ds in self.sets]
-        n_iter = len(self)
+        perms, n_iter = paired_epoch_plan(self.gen, [len(ds) for ds in self.sets], self.batch)
         ready: "queue.Queue" = queue.Queue()
         free = threading.Semaphore(self.depth)       # staging slots the producer may still fill
         stop = threading.Event()
@@ -280,7 +300,7 @@ class PairedFeatureLoader:
                     slot = self.buffers[it % self.depth]
                     sizes = []
                     for d, (ds, b) in enumerate(zip(self.sets, self.batch)):
-                        idx = perms[d][it * b:(it + 1) * b]
+                        idx = epoch_batch(perms[d], it, b)
                         ds.gather(idx, slot[d][0], slot[d][1])
                         sizes.append(len(idx))
                     ready.put((it, sizes))
@@ -305,6 +325,132 @@ class PairedFeatureLoader:
         finally:
             stop.set()
             worker.join(timeout=5)
+
+
+# ---- device-resident shards ------------------------------------------------------------------------------
+class DeviceFeatureBank:
+    """The rows of a `PackedTSNDataSet` in device memory, uploaded once: `features` is `(videos, T*feat_dim)` fp32 on
+    `device` (each distinct video once; `order` maps dataset positions -- num_dataload replication -- to rows, and
+    `labels` is in dataset order, as in the dataset).  The shard streams through ONE pinned staging buffer of
+    `chunk_bytes` (two halves, so that reading the next chunk overlaps the copy of the last); the memmap is never
+    pinned as a whole.  Before allocating, free device memory must cover the bank plus `headroom_bytes` (what the
+    training step and the rest of the process still need), otherwise `Ta3nError`."""
+
+    def __init__(self, dataset: PackedTSNDataSet, device=None, chunk_bytes: int = 64 << 20,
+                 headroom_bytes: int = 2 << 30):
+        from ._lib import Ta3nError
+        dev = torch.device(device if device is not None else "cuda")
+        if dev.type != "cuda":
+            raise Ta3nError("DeviceFeatureBank needs a CUDA device")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        src = dataset._rows
+        n, row_floats = int(src.shape[0]), int(src.shape[1])
+        if row_floats % 4:
+            raise Ta3nError(f"rows of {row_floats} floats are not 16-byte multiples; the device gather needs them")
+        nbytes = n * row_floats * 4
+        free, _ = torch.cuda.mem_get_info(dev)
+        cached = torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)   # this process may reuse it
+        if nbytes + int(headroom_bytes) > free + cached:
+            raise Ta3nError(f"feature bank of {nbytes / 2**30:.2f} GiB ({n} videos x {row_floats} floats) does not fit "
+                            f"on {dev}: {(free + cached) / 2**30:.2f} GiB free, {int(headroom_bytes) / 2**30:.2f} GiB "
+                            "kept for training; use the host pipeline (PairedFeatureLoader) for this dataset")
+        self.device = dev
+        self.row_shape = tuple(int(s) for s in dataset.features.shape[1:])
+        self.order = dataset.order
+        self.labels = dataset.labels
+        self.features = torch.empty((n, row_floats), device=dev, dtype=torch.float32)
+        per = max(1, int(chunk_bytes) // (2 * row_floats * 4))          # rows per half of the staging buffer
+        stage = torch.empty((2, per, row_floats), dtype=torch.float32, pin_memory=True)
+        done = [None, None]
+        with torch.cuda.device(dev):
+            for k, a in enumerate(range(0, n, per)):
+                h, b = k % 2, min(n, a + per)
+                if done[h] is not None:
+                    done[h].synchronize()               # the copy out of this half has finished
+                np.copyto(stage[h].numpy()[:b - a], src[a:b])
+                self.features[a:b].copy_(stage[h][:b - a], non_blocking=True)
+                done[h] = torch.cuda.Event()
+                done[h].record()
+            torch.cuda.current_stream().synchronize()
+
+    def __len__(self):
+        return int(self.order.shape[0])
+
+    @property
+    def nbytes(self) -> int:
+        return self.features.numel() * 4
+
+
+class DevicePairedSampler:
+    """`PairedFeatureLoader(source, target, batch_sizes, seed)` over two `DeviceFeatureBank`s: the same epochs (the
+    same `paired_epoch_plan`, one generator seeded once), but the batches are gathered on the device by the first
+    launch of the captured step that the sampler is handed to (`TrainStep(..., sampler=...)`, C ABI
+    `ta3n_gather_batch`).  `start_epoch()` draws the next epoch, uploads its row and label lists (outside the
+    graph, on the current stream), rewinds the device iteration index and returns the number of iterations; each
+    `TrainStep.run()` then consumes one of them."""
+
+    def __init__(self, source: DeviceFeatureBank, target: DeviceFeatureBank, batch_sizes: Sequence[int],
+                 seed: int = 0):
+        if source.device != target.device:
+            raise ValueError("both banks must live on the same device")
+        if source.row_shape != target.row_shape:
+            raise ValueError(f"source rows {source.row_shape} and target rows {target.row_shape} differ")
+        self.banks = (source, target)
+        self.batch = (int(batch_sizes[0]), int(batch_sizes[1]))
+        if min(self.batch) < 1:
+            raise ValueError("batch sizes must be >= 1")
+        self.device = source.device
+        self.row_shape = source.row_shape
+        self.lengths = (len(source), len(target))
+        self.gen = torch.Generator().manual_seed(seed)
+        dev = self.device
+        # fixed addresses, captured by the step's graph; zeros until the first epoch
+        self.rows = [torch.zeros(n, device=dev, dtype=torch.int32) for n in self.lengths]
+        self.labels = torch.zeros(self.lengths[0], device=dev, dtype=torch.int64)
+        self.state = torch.zeros(2, device=dev, dtype=torch.int32)      # {iteration, arrival counter}
+        self.n_iter = 0        # iterations of the current epoch (0 before the first start_epoch)
+        self.issued = 0        # of which run() has consumed
+
+    def __len__(self):
+        return paired_epoch_length(self.lengths, self.batch)
+
+    def start_epoch(self) -> int:
+        perms, n_iter = paired_epoch_plan(self.gen, self.lengths, self.batch)
+        for d, bank in enumerate(self.banks):
+            self.rows[d].copy_(torch.from_numpy(bank.order[perms[d]].astype(np.int32)))
+        self.labels.copy_(torch.from_numpy(self.banks[0].labels[perms[0]]))
+        self.rewind()
+        self.n_iter = n_iter
+        return n_iter
+
+    def rewind(self) -> None:
+        """Restart the current epoch at iteration 0 (current stream)."""
+        self.state.zero_()
+        self.issued = 0
+
+    def take(self) -> None:
+        """Account for one more iteration of the epoch; raises past its end (host-side, before anything runs)."""
+        if self.issued >= self.n_iter:
+            raise RuntimeError(f"the epoch has {self.n_iter} iterations and all have run; call start_epoch()"
+                               if self.n_iter else "call start_epoch() before the first run()")
+        self.issued += 1
+
+    def enqueue_gather(self, xs: torch.Tensor, xt: torch.Tensor, labels: torch.Tensor, valid: torch.Tensor,
+                       stream: int) -> None:
+        """Fill one input slot (source / target features, source labels, {real source rows, real target rows})
+        with the current iteration's batch and advance the device iteration index: one launch."""
+        from . import _lib
+        (bs, bt), (s, t) = self.batch, self.banks
+        if (xs.shape[0], xt.shape[0]) != (bs, bt) or tuple(xs.shape[1:]) != self.row_shape or \
+                tuple(xt.shape[1:]) != self.row_shape:
+            raise ValueError(f"slot {tuple(xs.shape)} + {tuple(xt.shape)} does not match the sampler's batches "
+                             f"{bs} + {bt} of {self.row_shape}")
+        _lib.check(_lib.load().ta3n_gather_batch(
+            s.features.data_ptr(), s.features.shape[0], self.rows[0].data_ptr(), self.labels.data_ptr(),
+            self.lengths[0], bs, xs.data_ptr(), labels.data_ptr(),
+            t.features.data_ptr(), t.features.shape[0], self.rows[1].data_ptr(), self.lengths[1], bt, xt.data_ptr(),
+            s.features.shape[1], valid.data_ptr(), self.state.data_ptr(), stream))
 
 
 def _main(argv=None):

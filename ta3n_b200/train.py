@@ -119,7 +119,7 @@ class TrainStep:
                  overlap_allreduce: Optional[bool] = None, graph_collectives: Optional[bool] = None,
                  optimizer: Optional[SGDNesterov] = None, mode: Optional[str] = None,
                  class_weight: Optional[torch.Tensor] = None, domain_weight: Sequence[float] = (1.0, 1.0),
-                 allreduce: Optional[str] = None, mu: float = 0.0):
+                 allreduce: Optional[str] = None, mu: float = 0.0, sampler=None):
         """mode: 'legacy' (default) = the per-operator sequence (25 launches in one CUDA graph; the only mode that
         supports use_attn_frame); 'phased' = the step program as 14 launches (ta3n_step_run_phased; default when class /
         domain weights or a scheduled beta are given).  class_weight / domain_weight: the weights of criterion /
@@ -139,9 +139,25 @@ class TrainStep:
         models.py:682-684); with mu == 0 its backward stops at the classifiers.  The two passes' gradients are summed
         before the all-reduce, clipping and SGD.  dis_MCD averages over the real target rows of the batch; a batch
         with no real target row contributes 0 (the reference would take the mean of an empty tensor).
-        mu: the GRL coefficient of pass 2 (--mu, fixed at capture); non-zero only under MCD."""
+        mu: the GRL coefficient of pass 2 (--mu, fixed at capture); non-zero only under MCD.
+
+        sampler: a ``dataset.DevicePairedSampler`` over feature banks in device memory.  Its gather is then the first
+        launch of every step (one launch more, in every mode, with or without the graph), each ``run()`` consumes one
+        iteration of the sampler's current epoch (``start_epoch()``) and raises past its end, and ``load()`` /
+        ``prefetch()`` / ``__call__`` raise.  Single rank only, and without ``double_buffer`` (nothing is left to
+        overlap)."""
         if not model.training:
             raise ValueError("TrainStep needs model.train() (dropout state is fixed at construction)")
+        if sampler is not None:
+            if double_buffer:
+                raise ValueError("double_buffer overlaps host-to-device copies; with a device sampler there are none")
+            if (dist.get_world_size(process_group) if dist.is_initialized() else 1) > 1:
+                # a short last global batch needs a rule for weighting the ranks' means, and a rank may get no real row
+                raise NotImplementedError("the device sampler feeds a single rank; with several ranks use "
+                                          "PairedFeatureLoader + load() / prefetch()")
+            if (int(sampler.batch[0]), int(sampler.batch[1])) != (int(batch_source), int(batch_target)):
+                raise ValueError(f"sampler batches {sampler.batch} != TrainStep({batch_source}, {batch_target})")
+        self.sampler = sampler
         ens = getattr(model, "ens_DA", "none")
         if model.use_attn == "general" or ens not in ("none", "MCD") or model.frame_aggregation != "trn-m":
             # the off-path variants (SURVEY 8f n4) run through VideoModel.forward + autograd; the captured step covers
@@ -169,6 +185,9 @@ class TrainStep:
         self.device = dev
         self.Bs, self.Bt = int(batch_source), int(batch_target)
         self.T, self.D = model.train_segments, model.feature_dim
+        if sampler is not None and (sampler.device != dev or tuple(sampler.row_shape) != (self.T, self.D)):
+            raise ValueError(f"sampler rows {tuple(sampler.row_shape)} on {sampler.device} do not match the model's "
+                             f"({self.T}, {self.D}) on {dev}")
         self.M, self.R = self.Bs + self.Bt, self.T - 1
         self.C = model.fc_classifier_video_source.weight.shape[0]
         self.gamma = float(gamma)
@@ -328,6 +347,8 @@ class TrainStep:
                 self.graphs[slot] = self._capture()
             self.active = 0
             self.xs, self.xt, self.labels, self.valid = self.slots[0]
+        if sampler is not None:
+            sampler.rewind()        # the capture's warm-up ran one gather
 
     def _init_mcd(self, seed, di, dv, offs):
         """State of MCD's second pass: its dropout seeds, buffers, and a second gradient bucket with the bucket's
@@ -571,6 +592,8 @@ class TrainStep:
             check(lib.ta3n_set_forward_scratch(None, 0))
 
     def _enqueue_body(self, lib, st, at_split, optimizer):
+        if self.sampler is not None:
+            self.sampler.enqueue_gather(self.xs, self.xt, self.labels, self.valid, st)     # this iteration's batch
         if self.mode != "legacy":
             check(lib.ta3n_step_run_phased(C.byref(self.step_descs[self.active][0]), st))
             if self.ar is not None:
@@ -745,11 +768,17 @@ class TrainStep:
 
     def load(self, source, target, labels):
         """Copy one paired mini-batch (host or device tensors) into the ACTIVE input slot (compute stream)."""
+        self._no_sampler("load")
         self._fill(self.active, source, target, labels)
+
+    def _no_sampler(self, what):
+        if self.sampler is not None:
+            raise RuntimeError(f"{what}() with a device sampler attached: run() gathers every batch itself")
 
     def prefetch(self, source, target, labels):
         """double_buffer=True: copy the NEXT mini-batch into the inactive slot on the copy stream, overlapping
         the step that is running; call ``swap()`` before the ``run()`` that should consume it."""
+        self._no_sampler("prefetch")
         if self.n_slots < 2:
             raise ValueError("prefetch needs TrainStep(double_buffer=True)")
         nxt = 1 - self.active
@@ -775,7 +804,9 @@ class TrainStep:
 
     def run(self):
         """forward + loss + backward (+ gradient all-reduce) (+ optimizer step when configured); returns the
-        device loss tensor (1,)."""
+        device loss tensor (1,).  With a device sampler the step first gathers the next batch of its epoch."""
+        if self.sampler is not None:
+            self.sampler.take()
         pending = None
         opt_done = self.opt is None
         if self.use_graph:
@@ -807,5 +838,6 @@ class TrainStep:
         return self.loss
 
     def __call__(self, source, target, labels):
+        self._no_sampler("__call__")
         self.load(source, target, labels)
         return self.run()
