@@ -291,6 +291,49 @@ int ta3n_gather_batch(const float* bank_s, long long n_rows_s, const int* rows_s
                       long long n_epoch_s, int batch_s, float* x_s, long long* y_s,
                       const float* bank_t, long long n_rows_t, const int* rows_t, long long n_epoch_t, int batch_t,
                       float* x_t, long long row_floats, int* valid_rows, unsigned int* state, ta3n_stream_t stream);
+/* The same gather for ONE labelled domain in a fixed order (validation: main.py:178 uses shuffle=False; the row list
+ * carries the num_dataload tiling): the rows of epoch positions [i*batch, min((i+1)*batch, n_epoch)) go to x
+ * [batch, row_floats], their labels to y [batch], the rest is zero-filled with label 0, valid_rows [1] = the number of
+ * real rows (what ta3n_eval_head reads), and state [2] advances as in ta3n_gather_batch.  Kernel label "gather_rows". */
+int ta3n_gather_rows(const float* bank, long long n_rows, const int* rows, const long long* labels, long long n_epoch,
+                     int batch, float* x, long long* y, long long row_floats, int* valid_rows, unsigned int* state,
+                     ta3n_stream_t stream);
+
+/* ---- validation head (main.py:707-730 validate(), test_models.py:115-193) ------------------------------------- */
+/* Epoch accumulator in device memory (8-byte aligned; zero it to start an epoch).                                  */
+typedef struct {
+  double loss_sum;            /* sum over batches of n_b * loss_b (losses.update(loss.item(), n_b), main.py:728)      */
+  long long n;                /* real rows seen                                                                      */
+  long long correct[4];       /* real rows whose label ranks below k[i]                                              */
+  int batch;                  /* launches folded in so far (the batch index of the next launch)                     */
+  unsigned int arrive;        /* arrival counter of the launch, 0 between launches                                  */
+} ta3n_eval_accum;
+
+size_t ta3n_eval_workspace_bytes(int rows);
+/* One launch per validation batch of `rows` rows, of which the first *valid_rows (device int) are real (the rest is
+ * the zero padding main.py:690-693 adds and removeDummy drops, :710):
+ *   logits [rows,C] = feat_video [rows,H] Wc^T + bc, in fp32 FFMA whatever GEMM engine is selected (Wc staged in
+ *     shared memory when it fits, streamed through it otherwise);
+ *   per real row r with label y = labels[r] (int64):  ce = logsumexp(z) - z_y (shifted by the max, summed in fp64);
+ *     w_y = class_weight[y] (class_weight may be NULL: 1);  rank = #{j : z_j > z_y} + #{j < y : z_j == z_y}, i.e.
+ *     TIES RANK BY CLASS INDEX (torch.topk leaves their order unspecified; this pins it);  correct@k = rank < k;
+ *     top-1 = the lowest index among the maxima (so top-1 == y exactly when rank == 0);
+ *   batch: loss_b = sum w_y ce / sum w_y over the real rows (CrossEntropyLoss(weight=...), main.py:205, 725), folded
+ *     into *accum as loss_sum += n_b * loss_b, n += n_b, correct[i] += its count for k_host[i] (n_k <= 4, 1 <= k <= C);
+ *     confusion [C,C] int64 (may be NULL) gets +1 at (y, top-1) per real row (test_models.py's cf);
+ *   epoch buffers (may be NULL): scores [n_epoch,C] and attn_out [n_epoch,R] receive the real rows' logits and
+ *     attention (row r of attn at attn + r*attn_ld, R floats) at row accum->batch * rows + r (dataset order when every
+ *     earlier batch was full); rows past n_epoch are dropped.
+ * A label outside [0, C), or a NaN among a row's logits, makes the batch loss NaN (as torch's criterion does for NaN)
+ * and that row counts at no k and in no confusion cell; it still counts in n.  A row of -inf logits is ordered by the
+ * rule above (every class ties: rank = y, top-1 = 0).  Per-CTA partials go to the workspace; the last
+ * CTA to arrive sums them in CTA order, folds them into *accum, advances accum->batch and re-arms accum->arrive, so
+ * reruns are bit-identical (no float atomics; the confusion counts are integer atomics).  Kernel label "eval_head". */
+int ta3n_eval_head(const float* feat_video, int rows, int H, int C, const float* Wc, const float* bc,
+                   const long long* labels, const float* class_weight, const int* valid_rows, int n_k,
+                   const int* k_host, const float* attn, int R, long long attn_ld, float* logits,
+                   ta3n_eval_accum* accum, long long* confusion, float* scores, float* attn_out, long long n_epoch,
+                   void* workspace, size_t workspace_bytes, ta3n_stream_t stream);
 
 /* ---- the training step as one step program (SURVEY 8a rows a1-a13 + 8f row n1) ----------------------------- */
 /* main.py:418 (model forward, models.py:545-722 trn-m branch), main.py:446, 508-538, 559-562 (composed loss:

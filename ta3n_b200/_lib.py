@@ -107,6 +107,10 @@ SIGNATURES = {
     "ta3n_accumulate": (_I, [_VP, _VP, C.c_longlong, _VP]),
     "ta3n_gather_batch": (_I, [_VP, C.c_longlong, _VP, _VP, C.c_longlong, _I, _VP, _VP,
                                _VP, C.c_longlong, _VP, C.c_longlong, _I, _VP, C.c_longlong, _VP, _VP, _VP]),
+    "ta3n_gather_rows": (_I, [_VP, C.c_longlong, _VP, _VP, C.c_longlong, _I, _VP, _VP, C.c_longlong, _VP, _VP, _VP]),
+    "ta3n_eval_workspace_bytes": (_SZ, [_I]),
+    "ta3n_eval_head": (_I, [_VP, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _I, _IP, _VP, _I, C.c_longlong, _VP,
+                            _VP, _VP, _VP, _VP, C.c_longlong, _VP, _SZ, _VP]),
     "ta3n_step_workspace_bytes": (_SZ, [C.POINTER(StepDesc)]),
     "ta3n_step_run_phased": (_I, [C.POINTER(StepDesc), _VP]),
     "ta3n_allreduce_flag_bytes": (_SZ, [_I]),

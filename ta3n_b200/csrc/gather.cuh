@@ -39,7 +39,7 @@ __device__ __forceinline__ float4 ld_stream_f4(const float4* p, uint64_t pol) {
 }
 
 // grid = (ceil(row_f4 / kGatherChunk), Bs + Bt): blockIdx.y is the slot row (source rows first), blockIdx.x a 16 KB
-// chunk of it.  state[0] is the iteration i, state[1] an arrival counter that is 0 between launches.  Slot row k of
+// chunk of it (ta3n_gather_rows passes a target domain of batch 0).  state[0] is the iteration i, state[1] an arrival counter that is 0 between launches.  Slot row k of
 // a domain takes epoch position i*batch + k; past the end of the epoch it is zero-filled (main.py:359-364 pads with
 // zero dummies).  Every CTA reads state[0] once before it arrives; the last CTA to arrive -- when no CTA can still be
 // reading it -- advances the iteration and re-arms the counter, so the index moves once per launch without a launch
@@ -67,7 +67,7 @@ gather_batch_kernel(const __grid_constant__ GatherDomain src, const __grid_const
     if (blockIdx.x == 0 && blockIdx.y == 0) {
       const long long ns = src.n_epoch - (long long)it * src.batch, nt = tgt.n_epoch - (long long)it * tgt.batch;
       valid_rows[0] = (int)max(0ll, min(ns, (long long)src.batch));
-      valid_rows[1] = (int)max(0ll, min(nt, (long long)tgt.batch));
+      if (tgt.batch > 0) valid_rows[1] = (int)max(0ll, min(nt, (long long)tgt.batch));   // one domain: one count
     }
   }
   __syncthreads();

@@ -896,6 +896,7 @@ struct DeviceInfo {
   int sm_count = 0;
   bool configured[4] = {false, false, false, false};        // seg_gemm_tc_kernel, per operand layout
   bool x3_configured[4] = {false, false, false, false};      // seg_gemm_tc_x3_kernel, per operand layout
+  bool eval_configured = false;                              // eval_head_kernel (eval.cuh)
 };
 inline std::mutex& device_mu() {
   static std::mutex mu;

@@ -9,6 +9,7 @@
 #include "step_plan.cuh"
 #include "allreduce.cuh"
 #include "gather.cuh"
+#include "eval.cuh"
 
 #include <functional>
 
@@ -1007,6 +1008,84 @@ int ta3n_gather_batch(const float* bank_s, long long n_rows_s, const int* rows_s
   TA3N_REQUIRE(grid.x <= 65535u, "rows too long");
   pre_launch("gather_batch", S(stream));
   launch_kernel(gather_batch_kernel, grid, kGatherThreads, 0, S(stream), s, t, row_f4, valid_rows, state);
+  return after_launch();
+}
+
+int ta3n_gather_rows(const float* bank, long long n_rows, const int* rows, const long long* labels, long long n_epoch,
+                     int batch, float* x, long long* y, long long row_floats, int* valid_rows, unsigned int* state,
+                     ta3n_stream_t stream) {
+  TA3N_REQUIRE(batch >= 1 && batch <= 65535, "batch must be in [1, 65535]");
+  TA3N_REQUIRE(row_floats >= 4 && row_floats % 4 == 0, "row_floats must be a positive multiple of 4 (16-byte rows)");
+  TA3N_REQUIRE(n_epoch >= 1, "empty epoch");
+  TA3N_REQUIRE(n_rows >= 1 && n_rows <= INT32_MAX, "bank rows must be in [1, 2^31) (row lists are int32)");
+  TA3N_REQUIRE(n_rows <= INT64_MAX / row_floats, "bank too large");
+  TA3N_REQUIRE(bank && rows && labels && x && y, "null pointer");
+  TA3N_REQUIRE(valid_rows && state, "null valid_rows / state");
+  TA3N_REQUIRE(aligned16(bank) && aligned16(x), "bank and slot must be 16-byte aligned");
+  GatherDomain s{reinterpret_cast<const float4*>(bank), n_rows, rows, labels, n_epoch, reinterpret_cast<float4*>(x),
+                 y, batch};
+  GatherDomain none{nullptr, 0, nullptr, nullptr, 0, nullptr, nullptr, 0};     // batch 0: no slot row, no count
+  const long long row_f4 = row_floats / 4;
+  const dim3 grid((unsigned)((row_f4 + kGatherChunk - 1) / kGatherChunk), (unsigned)batch);
+  TA3N_REQUIRE(grid.x <= 65535u, "rows too long");
+  pre_launch("gather_rows", S(stream));
+  launch_kernel(gather_batch_kernel, grid, kGatherThreads, 0, S(stream), s, none, row_f4, valid_rows, state);
+  return after_launch();
+}
+
+// ------------------------------------------------------------------------------------------------
+// validation head (include/ta3n_b200.h: ta3n_eval_head)
+// ------------------------------------------------------------------------------------------------
+static int eval_grid(int rows) { return (rows + kEvalRows - 1) / kEvalRows; }
+
+size_t ta3n_eval_workspace_bytes(int rows) {
+  return rows < 1 ? 0 : Arena::round((size_t)eval_grid(rows) * sizeof(EvalPartial));
+}
+
+int ta3n_eval_head(const float* feat_video, int rows, int H, int C, const float* Wc, const float* bc,
+                   const long long* labels, const float* class_weight, const int* valid_rows, int n_k,
+                   const int* k_host, const float* attn, int R, long long attn_ld, float* logits,
+                   ta3n_eval_accum* accum, long long* confusion, float* scores, float* attn_out, long long n_epoch,
+                   void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
+  TA3N_REQUIRE(rows >= 1 && H >= 1 && C >= 1, "rows, H and C must be >= 1");
+  TA3N_REQUIRE(n_k >= 1 && n_k <= kEvalMaxK && k_host, "between 1 and 4 top-k values");
+  for (int i = 0; i < n_k; ++i)
+    if (k_host[i] < 1 || k_host[i] > C)
+      return fail(TA3N_ERR_INVALID, "ta3n_eval_head: top-k value %d is outside [1, C=%d]", k_host[i], C);
+  TA3N_REQUIRE(feat_video && Wc && bc && labels && valid_rows && logits && accum, "null pointer");
+  TA3N_REQUIRE(reinterpret_cast<uintptr_t>(accum) % 8 == 0 && reinterpret_cast<uintptr_t>(confusion) % 8 == 0,
+               "accum and confusion must be 8-byte aligned");
+  TA3N_REQUIRE(!(scores || attn_out) || n_epoch >= 1, "epoch buffers need n_epoch >= 1");
+  TA3N_REQUIRE(!attn_out || (attn && R >= 1 && attn_ld >= R), "attn_out needs attn [rows, R] with attn_ld >= R");
+  const int grid = eval_grid(rows);
+  const size_t need = ta3n_eval_workspace_bytes(rows);
+  TA3N_REQUIRE(workspace && reinterpret_cast<uintptr_t>(workspace) % 16 == 0, "null or misaligned workspace");
+  if (workspace_bytes < need)
+    return fail(TA3N_ERR_WORKSPACE, "ta3n_eval_head: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+  const size_t x_bytes = (size_t)kEvalRows * H * sizeof(float), w_row = (size_t)(H + 1) * sizeof(float);
+  if (x_bytes + w_row > kEvalSmemBudget)
+    return fail(TA3N_ERR_UNSUPPORTED, "ta3n_eval_head: H=%d is too wide for the shared-memory staging", H);
+  EvalArgs a;
+  a.feat = feat_video, a.Wc = Wc, a.bc = bc, a.labels = labels, a.class_weight = class_weight;
+  a.valid_rows = valid_rows, a.attn = attn, a.logits = logits, a.accum = accum, a.confusion = confusion;
+  a.scores = scores, a.attn_out = attn_out, a.n_epoch = n_epoch, a.attn_ld = attn_ld;
+  a.rows = rows, a.H = H, a.C = C, a.R = R, a.n_k = n_k;
+  a.c_tile = (int)std::min<size_t>((size_t)C, (kEvalSmemBudget - x_bytes) / w_row);
+  for (int i = 0; i < kEvalMaxK; ++i) a.k[i] = i < n_k ? k_host[i] : 0;
+  const size_t smem = x_bytes + (size_t)a.c_tile * w_row;
+  {
+    std::lock_guard<std::mutex> lock(device_mu());
+    DeviceInfo* d = device_info();
+    if (!d) return fail(TA3N_ERR_CUDA, "cudaGetDevice failed");
+    if (!d->eval_configured) {
+      TA3N_CUDA(cudaFuncSetAttribute(eval_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)kEvalSmemBudget));
+      d->eval_configured = true;
+    }
+  }
+  pre_launch("eval_head", S(stream));
+  launch_kernel(eval_head_kernel, grid, kEvalThreads, smem, S(stream), a,
+                reinterpret_cast<EvalPartial*>(workspace));
   return after_launch();
 }
 

@@ -13,7 +13,8 @@ This module offers
   `RandomSampler` order, assembling every paired mini-batch directly into (pinned) staging buffers on a
   background thread, ready for `TrainStep.prefetch()`;
 * `DeviceFeatureBank` + `DevicePairedSampler`: the same epochs with the shards resident in device memory; each
-  mini-batch is gathered by the first launch of the captured step (`TrainStep(..., sampler=...)`).
+  mini-batch is gathered by the first launch of the captured step (`TrainStep(..., sampler=...)`);
+* `DeviceEvalSampler`: the validation loader (one bank, dataset order) for `evaluate.EvalStep(..., sampler=...)`.
 
 Both paired paths draw their epochs from `paired_epoch_plan`, so that one seed gives the same batches on either.
 """
@@ -451,6 +452,67 @@ class DevicePairedSampler:
             self.lengths[0], bs, xs.data_ptr(), labels.data_ptr(),
             t.features.data_ptr(), t.features.shape[0], self.rows[1].data_ptr(), self.lengths[1], bt, xt.data_ptr(),
             s.features.shape[1], valid.data_ptr(), self.state.data_ptr(), stream))
+
+
+class DeviceEvalSampler:
+    """The validation loader of main.py:176-178 (`shuffle=False`, `batch_size[2]`) over one `DeviceFeatureBank`: the
+    dataset positions in order, `ceil(N / batch)` batches, the last one short.  Each batch is gathered on the device
+    by the first launch of the captured validation step (`EvalStep(..., sampler=...)`, C ABI `ta3n_gather_rows`).
+    `start_epoch()` uploads the row list once (`bank.order`: the num_dataload tiling) and rewinds; each
+    `EvalStep` replay then consumes one batch."""
+
+    def __init__(self, bank: DeviceFeatureBank, batch: int):
+        if int(batch) < 1:
+            raise ValueError("batch size must be >= 1")
+        self.bank = bank
+        self.batch = int(batch)
+        self.device = bank.device
+        self.row_shape = bank.row_shape
+        self.n = len(bank)
+        dev = self.device
+        # fixed addresses, captured by the step's graph
+        self.rows = torch.zeros(self.n, device=dev, dtype=torch.int32)
+        self.labels = torch.zeros(self.n, device=dev, dtype=torch.int64)
+        self.state = torch.zeros(2, device=dev, dtype=torch.int32)      # {batch index, arrival counter}
+        self.uploaded = False
+        self.n_iter = 0
+        self.issued = 0
+
+    def __len__(self):
+        return -(-self.n // self.batch)
+
+    def start_epoch(self) -> int:
+        if not self.uploaded:
+            self.rows.copy_(torch.from_numpy(self.bank.order.astype(np.int32)))
+            self.labels.copy_(torch.from_numpy(np.ascontiguousarray(self.bank.labels, dtype=np.int64)))
+            self.uploaded = True
+        self.rewind()
+        self.n_iter = len(self)
+        return self.n_iter
+
+    def rewind(self) -> None:
+        """Restart the epoch at batch 0 (current stream)."""
+        self.state.zero_()
+        self.issued = 0
+
+    def take(self) -> None:
+        """Account for one more batch of the epoch; raises past its end (host-side, before anything runs)."""
+        if self.issued >= self.n_iter:
+            raise RuntimeError(f"the epoch has {self.n_iter} batches and all have run; call start_epoch()"
+                               if self.n_iter else "call start_epoch() before the first run")
+        self.issued += 1
+
+    def enqueue_gather(self, x: torch.Tensor, labels: torch.Tensor, valid: torch.Tensor, stream: int) -> None:
+        """Fill the input slot (features, labels, {real rows}) with the current batch and advance the device batch
+        index: one launch."""
+        from . import _lib
+        if x.shape[0] != self.batch or tuple(x.shape[1:]) != self.row_shape:
+            raise ValueError(f"slot {tuple(x.shape)} does not match the sampler's batches of {self.batch} x "
+                             f"{self.row_shape}")
+        f = self.bank.features
+        _lib.check(_lib.load().ta3n_gather_rows(
+            f.data_ptr(), f.shape[0], self.rows.data_ptr(), self.labels.data_ptr(), self.n, self.batch, x.data_ptr(),
+            labels.data_ptr(), f.shape[1], valid.data_ptr(), self.state.data_ptr(), stream))
 
 
 def _main(argv=None):

@@ -239,10 +239,13 @@ class Buffers:
         return self.get("ws_" + name, max(int(nbytes), 256), dtype=torch.uint8)
 
 
-def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: bool = False):
+def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: bool = False,
+                 stop_at_video_feature: bool = False):
     """The six forward C calls of the path.  Returns (saved tensors dict, outputs tuple, dims).
     ``batch_gemms``: issue the frame-discriminator and TRN GEMMs (both read the shared features) as one
-    grouped launch (ta3n_fwd_batch_*); not applicable with frame attention, where TRN reads its output."""
+    grouped launch (ta3n_fwd_batch_*); not applicable with frame attention, where TRN reads its output.
+    ``stop_at_video_feature`` (validation): end at feat_video -- no video head, no video discriminator, and the frame
+    discriminator only when the frame attention reads it; the outputs those calls make are None."""
     lib = _lib.load()
     st = _stream()
     T = spec.num_segments
@@ -262,7 +265,7 @@ def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: boo
     check(lib.ta3n_shared_fc_fwd(_p(xs), Bs * T, _p(xt), Bt * T, D, _p(w_sh), _p(b_sh), F, _dref(d_i),
                                  _p(feat), st))
     # 2. frame-level discriminator  (models.py:606-610)
-    frame_disc = not spec.classify_only or spec.use_attn_frame
+    frame_disc = not (spec.classify_only or stop_at_video_feature) or spec.use_attn_frame
     hid_f = pred_frame = None
     batched = batch_gemms and not spec.use_attn_frame and frame_disc
     if batched:
@@ -300,12 +303,13 @@ def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: boo
         check(lib.ta3n_general_attn_fwd(_p(feat_rel), M, R, H, _p(wa1), _p(ba1), _p(wa2), _p(ba2), _p(hid_a), _p(attn),
                                         _p(feat_video), st))
     # 5. video head  (models.py:679-687)
-    dropped, pred_video = new("dropped", M, H), new("pred_video", M, Cn)
-    check(lib.ta3n_video_head_fwd(_p(feat_video), M, H, Cn, _p(w_c), _p(b_c), _dref(d_v), _p(dropped),
-                                  _p(pred_video), st))
+    dropped = pred_video = hid_v = pred_dom_video = None
+    if not stop_at_video_feature:
+        dropped, pred_video = new("dropped", M, H), new("pred_video", M, Cn)
+        check(lib.ta3n_video_head_fwd(_p(feat_video), M, H, Cn, _p(w_c), _p(b_c), _dref(d_v), _p(dropped),
+                                      _p(pred_video), st))
     # 6. video-level discriminator  (models.py:694-698)
-    hid_v = pred_dom_video = None
-    if not spec.classify_only:
+    if not (spec.classify_only or stop_at_video_feature):
         hid_v, pred_dom_video = new("hid_v", M, H), new("pred_dom_video", M, 2)
         check(lib.ta3n_disc_fwd(_p(dropped), M, H, H, _p(w1v), _p(b1v), _p(w2v), _p(b2v), _p(hid_v),
                                 _p(pred_dom_video), st))
@@ -491,10 +495,11 @@ def video_path(spec: PathSpec, xs: torch.Tensor, xt: torch.Tensor, params: Seque
 _AVG_OUT_NAMES = ("feat", "pred_frame", "feat_video", "pred_video", "pred_dom_video", "dropped")
 
 
-def avgpool_forward(spec: PathSpec, xs, xt, params, bufs: Buffers):
+def avgpool_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, stop_at_video_feature: bool = False):
     """models.py:557-610 (shared layer, frame discriminator), :427-432 (attention re-weighting + AvgPool2d([T,1])),
     :679-698 (dropout_v, classifier, video discriminator) as seven C calls.  ``spec.use_attn`` = use_attn='TransAttn':
-    the frame features are re-weighted by (1 - H(softmax(pred_frame)) + 1) before the average."""
+    the frame features are re-weighted by (1 - H(softmax(pred_frame)) + 1) before the average.
+    ``stop_at_video_feature`` as in path_forward: end at feat_video, the frame discriminator only under TransAttn."""
     lib = _lib.load()
     st = _stream()
     T = spec.num_segments
@@ -512,8 +517,11 @@ def avgpool_forward(spec: PathSpec, xs, xt, params, bufs: Buffers):
     d_i, d_v = spec.drop_i.cstruct(), spec.drop_v.cstruct()
     feat = new("feat", M * T, F)
     check(lib.ta3n_shared_fc_fwd(_p(xs), Bs * T, _p(xt), Bt * T, D, _p(w_sh), _p(b_sh), F, _dref(d_i), _p(feat), st))
-    hid_f, pred_frame = new("hid_f", M * T, F), new("pred_frame", M * T, 2)
-    check(lib.ta3n_disc_fwd(_p(feat), M * T, F, F, _p(w1f), _p(b1f), _p(w2f), _p(b2f), _p(hid_f), _p(pred_frame), st))
+    hid_f = pred_frame = None
+    if spec.use_attn or not stop_at_video_feature:
+        hid_f, pred_frame = new("hid_f", M * T, F), new("pred_frame", M * T, 2)
+        check(lib.ta3n_disc_fwd(_p(feat), M * T, F, F, _p(w1f), _p(b1f), _p(w2f), _p(b2f), _p(hid_f), _p(pred_frame),
+                                st))
     if spec.use_attn:
         feat_att = new("feat_att", M * T, F)
         check(lib.ta3n_frame_attn_fwd(_p(feat), _p(pred_frame), M * T, F, _p(feat_att), st))
@@ -521,6 +529,11 @@ def avgpool_forward(spec: PathSpec, xs, xt, params, bufs: Buffers):
         feat_att = feat
     feat_video = new("feat_video", M, F)
     check(lib.ta3n_segment_mean_fwd(_p(feat_att), M, T, F, _p(feat_video), st))
+    if stop_at_video_feature:
+        saved = dict(feat=feat, hid_f=hid_f, pred_frame=pred_frame, dropped=None, hid_v=None)
+        outputs = (feat.view(M, T, F), None if pred_frame is None else pred_frame.view(M, T, 2), feat_video, None,
+                   None, None)
+        return saved, outputs, (Bs, Bt, D, T, F, Cn)
     dropped, pred_video = new("dropped", M, F), new("pred_video", M, Cn)
     check(lib.ta3n_video_head_fwd(_p(feat_video), M, F, Cn, _p(w_c), _p(b_c), _dref(d_v), _p(dropped), _p(pred_video), st))
     hid_v, pred_dom_video = new("hid_v", M, F), new("pred_dom_video", M, 2)
