@@ -5,8 +5,9 @@ The reference needs three environment shims to import under this image
   1. ``colorama`` is imported at models.py:11-12 but not installed -> stub module;
   2. models.py:14 uses the bare name ``torch`` which it expected to leak from
      ``from torch.nn.init import *`` (models.py:3) -> publish it through builtins;
-  3. models.py:125 builds ``torchvision.models.resnet101(True)`` only to read
-     ``fc.in_features`` (would download weights; no network) -> tiny stand-in.
+  3. models.py:125 builds ``torchvision.models.<base_model>(True)`` only to read
+     ``fc.in_features`` (would download weights; no network) -> tiny stand-ins that
+     report the pool5 width: 2048 for resnet101, 512 for resnet18 / resnet34.
 
 ``/root/reference`` exists only in the build container, never on the GPU box;
 callers must check ``available()`` first.
@@ -65,11 +66,12 @@ def load():
         sys.modules["colorama"] = stub
     builtins.torch = torch
 
-    class _HeadOnly:
-        class fc:
-            in_features = 2048
+    def head_only(width):
+        fc = type("fc", (), {"in_features": width})
+        return lambda *a, **k: type("HeadOnly", (), {"fc": fc})()
 
-    torchvision.models.resnet101 = lambda *a, **k: _HeadOnly()
+    for name, width in (("resnet101", 2048), ("resnet18", 512), ("resnet34", 512)):
+        setattr(torchvision.models, name, head_only(width))
 
     if root not in sys.path:
         sys.path.insert(0, root)

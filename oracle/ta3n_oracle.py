@@ -59,6 +59,7 @@ class PathConfig:
     use_attn_frame: str = "none"   # or 'TransAttn'
     ens_DA: str = "none"           # or 'MCD': a second video-level classifier (models.py:276-279, 716-720)
     frame_aggregation: str = "trn-m"   # or 'avgpool' (models.py:240-241, 425-433, 620-626): no relation level
+    feature_dim: int = FEATURE_DIM     # input width D: 2048 for resnet50/101/152, 512 for resnet18/34 (models.py:125-126)
 
     @property
     def video_dim(self) -> int:    # feat_aggregated_dim = feat_video_dim, models.py:240-250
@@ -66,7 +67,7 @@ class PathConfig:
 
     @property
     def shared_dim(self) -> int:   # models.py:129
-        return min(self.fc_dim, FEATURE_DIM)
+        return min(self.fc_dim, self.feature_dim)
 
 
 # ----------------------------------------------------------------------------
@@ -127,7 +128,7 @@ def init_params(cfg: PathConfig, seed: Optional[int] = None) -> "OrderedDict[str
     def put(name, wb):
         p[name + ".weight"], p[name + ".bias"] = wb
 
-    put("fc_feature_shared_source", _std_linear(FEATURE_DIM, Fd))
+    put("fc_feature_shared_source", _std_linear(cfg.feature_dim, Fd))
     put("fc_feature_source", _std_linear(Fd, Fd))               # registered, unused (App. C)
     put("fc_feature_domain", _std_linear(Fd, Fd))
     put("fc_classifier_source", _std_linear(Fd, C))             # executed, output dropped
@@ -514,10 +515,10 @@ def train_step(params: Dict[str, torch.Tensor], xs, xt, labels, beta, cfg: PathC
 
 
 def synthetic_batch(batch: int, cfg: PathConfig, seed: int = 4321, dtype=torch.float32):
-    """Synthetic (B,T,2048) N(0,1) features and labels arange(B) % C (SURVEY §8d)."""
+    """Synthetic (B,T,D) N(0,1) features and labels arange(B) % C (SURVEY §8d)."""
     g = torch.Generator().manual_seed(seed)
-    xs = torch.randn(batch, cfg.num_segments, FEATURE_DIM, generator=g).to(dtype)
-    xt = torch.randn(batch, cfg.num_segments, FEATURE_DIM, generator=g).to(dtype)
+    xs = torch.randn(batch, cfg.num_segments, cfg.feature_dim, generator=g).to(dtype)
+    xt = torch.randn(batch, cfg.num_segments, cfg.feature_dim, generator=g).to(dtype)
     labels = torch.arange(batch) % cfg.num_class
     return xs, xt, labels
 

@@ -8,39 +8,42 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import gen_golden
+from oracle import gen_golden, gen_golden_widths
 from oracle import ta3n_oracle as orc
 from tests.golden_util import STRUCTURAL_ZERO_GRADS, TOL_FP32, assert_close
 
-PINS = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_pins.npz"))
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+PINS = np.load(os.path.join(GOLDEN, "reference_pins.npz"))
 META = json.loads(bytes(PINS["meta_json"]).decode())
+WIDTH_PINS = np.load(os.path.join(GOLDEN, "width_pins.npz"))
+WIDTH_META = json.loads(bytes(WIDTH_PINS["meta_json"]).decode())
 
 
-def assert_pinned(t, key, tol, what):
+def assert_pinned(t, key, tol, what, pins=PINS):
     """Compare with a stored reference tensor: whole when small, else its sum / norm and a strided sample."""
     t = t.detach().double().cpu()
-    if key in PINS.files:
-        want = PINS[key]
+    if key in pins.files:
+        want = pins[key]
         assert tuple(t.shape) == want.shape, (what, tuple(t.shape), want.shape)
         assert_close(t, want, tol, what)
         return
-    s, n = PINS[key + "#stats"]
+    s, n = pins[key + "#stats"]
     flat = t.reshape(-1)
     assert abs(flat.norm().item() - n) <= tol * n, f"{what}: norm {flat.norm().item():.6e} vs {n:.6e}"
     assert abs(flat.sum().item() - s) <= tol * max(n, abs(s)) * 4, f"{what}: sum {flat.sum().item():.6e} vs {s:.6e}"
-    assert_close(flat[::META["stride"]], PINS[key + "#sample"], tol * 4, what + " (sample)")
+    assert_close(flat[::META["stride"]], pins[key + "#sample"], tol * 4, what + " (sample)")
 
 
-def assert_pinned_equal(t, key, what):
+def assert_pinned_equal(t, key, what, pins=PINS):
     """Bit-level equality with a stored reference tensor (init values)."""
     t = t.detach().double().cpu()
-    if key in PINS.files:
-        assert torch.equal(t, torch.from_numpy(PINS[key])), what
+    if key in pins.files:
+        assert torch.equal(t, torch.from_numpy(pins[key])), what
         return
-    s, n = PINS[key + "#stats"]
+    s, n = pins[key + "#stats"]
     flat = t.reshape(-1)
     assert abs(flat.norm().item() - n) <= 1e-12 * max(1.0, n) and abs(flat.sum().item() - s) <= 1e-12 * max(1.0, n), what
-    assert torch.equal(flat[::META["stride"]], torch.from_numpy(PINS[key + "#sample"])), what
+    assert torch.equal(flat[::META["stride"]], torch.from_numpy(pins[key + "#sample"])), what
 
 
 @pytest.mark.parametrize("case", ["cfg1_train_masked", "t9_attnframe", "noattn_f256", "general_attn", "avgpool_transattn",
@@ -64,6 +67,34 @@ def test_oracle_equals_live_reference(case):
             assert float(grads[name].norm()) < 1e-6
         else:
             assert_pinned(grads[name], k + "grad/" + name, 2e-4, f"grad {name}")
+
+
+@pytest.mark.parametrize("case", list(gen_golden_widths.CASES))
+def test_oracle_equals_live_reference_at_layer_widths(case):
+    """PathConfig.feature_dim and the shared widths the options allow: fc_dim 1024 (opts.py's default), fc_dim above
+    the input width (F = min(fc_dim, D) = 2048), resnet18's D = 512, and F = 250 off the float4 grid.  The oracle's
+    initial state_dict equals the reference's bit for bit (same keys, shapes and values under one seed), and one
+    training step on injected dropout masks gives the reference's loss, outputs and gradients."""
+    c = gen_golden_widths.CASES[case]
+    cfg, xs, xt, labels, masks = gen_golden_widths.case_inputs(c)
+    k = f"{case}/"
+    params = orc.init_params(cfg, seed=gen_golden.MODEL_SEED)
+    assert list(params.keys()) == WIDTH_META[k + "init/keys"]
+    for (name, v), shape in zip(params.items(), WIDTH_META[k + "init/shapes"]):
+        assert list(v.shape) == shape, name
+        assert_pinned_equal(v, k + "init/" + name, name, pins=WIDTH_PINS)
+    assert params["fc_feature_shared_source.weight"].shape == (cfg.shared_dim, cfg.feature_dim)
+    loss, outs, grads = orc.train_step(params, xs, xt, labels, gen_golden.BETA, cfg, gen_golden.GAMMA,
+                                       train=True, masks=masks)
+    assert_pinned(loss, k + "loss", TOL_FP32, "loss", pins=WIDTH_PINS)
+    flat = [outs[0], outs[1], *outs[3], *outs[4], outs[5], outs[6], *outs[8], *outs[9]]
+    assert len(flat) == WIDTH_META[k + "n_out"]
+    for i, a in enumerate(flat):
+        assert_pinned(a, k + f"out{i}", TOL_FP32, f"output {i}", pins=WIDTH_PINS)
+    with_grad = WIDTH_META[k + "with_grad"]
+    assert sorted(grads) == sorted(with_grad)
+    for name in with_grad:
+        assert_pinned(grads[name], k + "grad/" + name, 2e-4, f"grad {name}", pins=WIDTH_PINS)
 
 
 def test_reference_state_dict_keys_match_oracle_init():
