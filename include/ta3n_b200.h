@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define TA3N_ABI_VERSION 5
+#define TA3N_ABI_VERSION 6
 
 enum {
   TA3N_OK = 0,
@@ -437,6 +437,27 @@ int ta3n_sgd_nesterov_step_masked(float* params, const float* grads, float* mome
                                   const float* lr_dev, float momentum, float weight_decay, float max_norm,
                                   void* workspace, size_t workspace_bytes, float* stats, const float* active,
                                   ta3n_stream_t stream);
+
+/* main.py:578-581 clip_grad_norm_ followed by main.py:84-86 torch.optim.Adam(lr, betas=(beta1, beta2), eps,
+ * weight_decay).step() (L2 weight decay added to the gradient, amsgrad=False), over the same FLAT buffers (exp_avg and
+ * exp_avg_sq zero-initialised), in the order of torch's single-tensor implementation:
+ *     coef = min(1, max_norm / (||g||_2 + 1e-6))        (max_norm <= 0: no clipping, coef = 1)
+ *     t = *step_dev + 1;  bc1 = 1 - beta1^t;  bc2_sqrt = sqrt(1 - beta2^t);  step_size = lr / bc1
+ *     d = coef*g + weight_decay*p;  m += (1-beta1)*(d - m);  v = beta2*v + (1-beta2)*d*d
+ *     p -= step_size * m / (sqrt(v)/bc2_sqrt + eps)
+ * The scalars are computed in fp64 from t and the double betas (torch's Python floats) and rounded to fp32 once.
+ * *step_dev (device, the Adam step count t of every updated parameter) advances by one per call, inside the kernel,
+ * so a replayed CUDA graph applies the right bias correction.  lr is read from *lr_dev as for SGD; grads are not
+ * modified.  workspace: ta3n_adam_workspace_bytes(), zero-initialised before the first call (it holds an arrival
+ * counter that every call leaves at zero; one workspace per stream of concurrent calls).  stats and active as for
+ * ta3n_sgd_nesterov_step_masked: a masked element keeps p, m and v (torch skips parameters whose .grad is None).
+ * Requires 0 <= beta < 1, eps > 0, weight_decay >= 0, 16-byte aligned buffers.  Two launches (one without
+ * clipping); deterministic.                                                                                            */
+size_t ta3n_adam_workspace_bytes(void);
+int ta3n_adam_step_masked(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
+                          const float* lr_dev, uint64_t* step_dev, double beta1, double beta2, float eps,
+                          float weight_decay, float max_norm, void* workspace, size_t workspace_bytes, float* stats,
+                          const float* active, ta3n_stream_t stream);
 
 /* ---- self test of the tensor-core GEMM engine (used by tests; device buffers) ------ */
 /* C[M,N] = A[M,K] * B[N,K]^T with the selected engine; A, B, C row-major fp32.           */

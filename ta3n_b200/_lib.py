@@ -11,7 +11,7 @@ import threading
 
 from . import build as _build
 
-ABI_VERSION = 5     # TA3N_ABI_VERSION of include/ta3n_b200.h that SIGNATURES mirrors
+ABI_VERSION = 6     # TA3N_ABI_VERSION of include/ta3n_b200.h that SIGNATURES mirrors
 
 TA3N_GEMM_FP32_SIMT = 0
 TA3N_GEMM_TF32_TCGEN05 = 1
@@ -118,6 +118,9 @@ SIGNATURES = {
     "ta3n_sgd_workspace_bytes": (_SZ, []),
     "ta3n_sgd_nesterov_step": (_I, [_VP, _VP, _VP, C.c_longlong, _VP, _F, _F, _F, _VP, _SZ, _VP, _VP]),
     "ta3n_sgd_nesterov_step_masked": (_I, [_VP, _VP, _VP, C.c_longlong, _VP, _F, _F, _F, _VP, _SZ, _VP, _VP, _VP]),
+    "ta3n_adam_workspace_bytes": (_SZ, []),
+    "ta3n_adam_step_masked": (_I, [_VP, _VP, _VP, _VP, C.c_longlong, _VP, _VP, C.c_double, C.c_double, _F, _F, _F,
+                                   _VP, _SZ, _VP, _VP, _VP]),
     "ta3n_gemm_tn": (_I, [_VP, _VP, _VP, _I, _I, _I, _VP]),
     "ta3n_gemm_ex": (_I, [_VP, _I, _I, _VP, _I, _I, _VP, _I, _I, _I, _I, _VP, _SZ, _VP]),
 }

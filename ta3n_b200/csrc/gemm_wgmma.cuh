@@ -942,8 +942,14 @@ inline int encode_map(const MapKey& k, CUtensorMap* out) {
   PFN_encodeTiled fn = encode_fn();
   if (!fn) return fail(TA3N_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   // a DRIVER call: the calling thread needs a current context.  A replica thread of nn.DataParallel (main.py:79) has
-  // only selected its device through the runtime so far -- bind the primary context (no-op when already bound).
-  cudaFree(nullptr);
+  // only selected its device through the runtime so far -- bind the primary context, once per thread: cudaFree is
+  // illegal while a stream is being captured, and a miss can happen inside a CUDA graph capture (after the clear
+  // below, keys its warm-up encoded are gone)
+  static thread_local bool context_bound = false;
+  if (!context_bound) {
+    cudaFree(nullptr);
+    context_bound = true;
+  }
   cuuint64_t dims[3] = {(cuuint64_t)k.inner, (cuuint64_t)k.outer, 1};
   cuuint64_t strides[2] = {(cuuint64_t)k.ld * sizeof(float), 128};
   cuuint32_t box[3] = {(cuuint32_t)k.box_inner, (cuuint32_t)k.box_outer, 4};

@@ -1241,6 +1241,41 @@ int ta3n_sgd_nesterov_step(float* params, const float* grads, float* momentum_bu
                                        workspace_bytes, stats, nullptr, stream);
 }
 
+// ---- optimizer step: clip_grad_norm_ + Adam over flat buffers (main.py:84-86, 578-583) ----
+size_t ta3n_adam_workspace_bytes(void) {
+  return Arena::round(kSqnormBlocks * sizeof(float)) + Arena::round(sizeof(unsigned int));
+}
+
+int ta3n_adam_step_masked(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
+                          const float* lr_dev, uint64_t* step_dev, double beta1, double beta2, float eps,
+                          float weight_decay, float max_norm, void* workspace, size_t workspace_bytes, float* stats,
+                          const float* active, ta3n_stream_t stream) {
+  TA3N_REQUIRE(params && grads && exp_avg && exp_avg_sq && lr_dev && step_dev && n > 0, "bad arguments");
+  TA3N_REQUIRE(((reinterpret_cast<uintptr_t>(params) | reinterpret_cast<uintptr_t>(grads) |
+                 reinterpret_cast<uintptr_t>(exp_avg) | reinterpret_cast<uintptr_t>(exp_avg_sq)) & 15) == 0,
+               "flat buffers must be 16-byte aligned");
+  TA3N_REQUIRE(active == nullptr || (reinterpret_cast<uintptr_t>(active) & 15) == 0, "active mask must be 16-byte aligned");
+  TA3N_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "betas must lie in [0, 1)");
+  TA3N_REQUIRE(eps > 0.f && weight_decay >= 0.f, "eps must be positive and weight decay non-negative");
+  TA3N_REQUIRE(workspace != nullptr && workspace_bytes >= ta3n_adam_workspace_bytes() &&
+               (reinterpret_cast<uintptr_t>(workspace) & 3) == 0, "workspace too small");
+  float* partial = static_cast<float*>(workspace);
+  unsigned int* arrival = reinterpret_cast<unsigned int*>(static_cast<char*>(workspace) +
+                                                          Arena::round(kSqnormBlocks * sizeof(float)));
+  if (max_norm > 0.f) {
+    pre_launch("sqnorm", S(stream));
+    launch_kernel(sqnorm_partial_kernel, kSqnormBlocks, kOptThreads, 0, S(stream), grads, n, partial);
+    TA3N_TRY(after_launch());
+  }
+  long long n4 = (n + 3) / 4;
+  int blocks = static_cast<int>(std::min<long long>((n4 + kOptThreads - 1) / kOptThreads, 132 * 8));
+  pre_launch("adam", S(stream));
+  launch_kernel(adam_step_kernel, blocks, kOptThreads, 0, S(stream), params, grads, exp_avg, exp_avg_sq, n, lr_dev,
+                reinterpret_cast<unsigned long long*>(step_dev), beta1, beta2, eps, weight_decay, max_norm,
+                static_cast<const float*>(partial), kSqnormBlocks, arrival, stats, active);
+  return after_launch();
+}
+
 // ------------------------------------------------------------------------------------------------
 int ta3n_gemm_tn(const float* A, const float* B, float* C, int M, int N, int K, ta3n_stream_t stream) {
   TA3N_REQUIRE(A && B && C && M > 0 && N > 0 && K > 0, "bad arguments");

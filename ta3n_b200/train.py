@@ -25,7 +25,7 @@ import ctypes as C
 import os
 import math
 from dataclasses import dataclass
-from typing import List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 import torch.distributed as dist
@@ -49,6 +49,23 @@ class SGDNesterov:
     momentum: float = 0.9
     weight_decay: float = 1e-4
     clip_gradient: Optional[float] = 20.0
+
+
+@dataclass
+class Adam:
+    """``torch.optim.Adam(model.parameters(), lr, betas, eps, weight_decay)`` (main.py:84-86 with --optimizer Adam; L2
+    weight decay added to the gradient, amsgrad off) preceded by ``clip_grad_norm_(model.parameters(), clip_gradient)``
+    (main.py:578-581; None = no clipping), run as two kernels over the flat parameter / gradient / moment buffers (C ABI
+    ``ta3n_adam_step_masked``).  The defaults are torch's, except weight_decay: opts.py's default, which main.py:86
+    passes."""
+    lr: float
+    betas: Tuple[float, float] = (0.9, 0.999)
+    eps: float = 1e-8
+    weight_decay: float = 1e-4
+    clip_gradient: Optional[float] = 20.0
+
+
+Optimizer = Union[SGDNesterov, Adam]
 
 
 def lr_dann(lr0: float, p: float) -> float:
@@ -105,6 +122,143 @@ def flatten_parameters(model) -> torch.Tensor:
     return flat
 
 
+# ---- optimizer state in torch.optim's format ---------------------------------------------------------------------
+def _stock_optimizer(params, opt: Optimizer) -> torch.optim.Optimizer:
+    """The torch.optim optimizer main.py:83 / 84-86 builds for ``opt`` (it allocates no state until its first step)."""
+    if isinstance(opt, Adam):
+        return torch.optim.Adam(params, opt.lr, betas=tuple(opt.betas), eps=opt.eps, weight_decay=opt.weight_decay)
+    return torch.optim.SGD(params, opt.lr, momentum=opt.momentum, weight_decay=opt.weight_decay, nesterov=True)
+
+
+def _state_keys(opt: Optimizer) -> Tuple[str, ...]:
+    """Names of the per-parameter state buffers, as torch.optim calls them (one flat buffer each)."""
+    return ("exp_avg", "exp_avg_sq") if isinstance(opt, Adam) else ("momentum_buffer",)
+
+
+def _updated_slots(model, active: Optional[torch.Tensor]):
+    """(index in ``model.parameters()``, parameter, flat offset) of every tensor of the flat buffers that the fused
+    update touches (``active`` is the per-element mask of the update, None = all).  Parameters are matched by identity,
+    so MCD's second classifier, appended to the flat buffers, gets its index in ``model.parameters()``."""
+    params = step_parameters(model)
+    _, offs, _, _ = bucket_layout(params)
+    index = {id(p): i for i, p in enumerate(model.parameters())}
+    on = [True] * len(params) if active is None else \
+        (active[torch.tensor([offs[j] for j in range(len(params))], device=active.device)] != 0).tolist()
+    return [(index[id(p)], p, offs[j]) for j, p in enumerate(params) if on[j]]
+
+
+def optimizer_state_to_torch(model, opt: Optimizer, flat_state: Dict[str, torch.Tensor],
+                             active: Optional[torch.Tensor] = None, step: int = 0) -> dict:
+    """What ``torch.optim.SGD`` / ``Adam(model.parameters(), ...)`` with ``opt``'s hyper-parameters (main.py:83 / 86)
+    returns from ``state_dict()`` when its state is that of the flat buffers ``flat_state`` (by torch's state name:
+    'momentum_buffer', or 'exp_avg' and 'exp_avg_sq'; laid out as ``bucket_layout``).  One param group listing every
+    parameter of the model; state only for the parameters ``active`` lets the update touch, keyed by their index in
+    ``model.parameters()``.  ``step``: the Adam step count, for SGD any positive number once an update has run; 0
+    means no update yet, and the state is empty, as torch's is before its first step.  The state tensors are copies
+    that own their storage (a view would save the whole flat buffer and follow later steps).  Works on CPU tensors."""
+    # the param group as the installed torch writes it, from a stock optimizer over one host tensor (a torch.optim
+    # optimizer is freed by the cyclic garbage collector only: one over the model would keep the exported state's
+    # device memory alive until that runs)
+    group = _stock_optimizer([torch.zeros(1)], opt).state_dict()["param_groups"][0]
+    group["params"] = list(range(len(list(model.parameters()))))
+    state = {}
+    if step > 0:
+        keys = _state_keys(opt)
+        for i, p, off in sorted(_updated_slots(model, active), key=lambda s: s[0]):
+            entry = {k: flat_state[k][off:off + p.numel()].view_as(p).clone() for k in keys}
+            if isinstance(opt, Adam):
+                # torch.optim.Adam's step: a 0-dim float tensor on the host (non-capturable, non-fused path)
+                dtype = torch.float64 if torch.get_default_dtype() == torch.float64 else torch.float32
+                entry = {"step": torch.tensor(float(step), dtype=dtype), **entry}
+            state[i] = entry
+    return {"state": state, "param_groups": [group]}
+
+
+# switches that only some torch releases write into a param group; a group without one had it off
+_OPTIONAL_KEYS = ("maximize", "decoupled_weight_decay", "foreach", "capturable", "differentiable", "fused")
+# values the fused update implements, beside opt's own hyper-parameters (missing = the switch was off)
+_ADAM_FIXED = {"amsgrad": False, "maximize": False, "decoupled_weight_decay": False}
+_SGD_FIXED = {"dampening": 0, "nesterov": True, "maximize": False}
+
+
+def optimizer_state_from_torch(model, opt: Optimizer, sd: dict, flat_state: Dict[str, torch.Tensor],
+                               active: Optional[torch.Tensor] = None) -> Tuple[float, int]:
+    """Copy a torch.optim ``state_dict()`` -- from ``optimizer_state_to_torch`` or from a stock SGD / Adam built over
+    ``model.parameters()`` -- into the flat buffers ``flat_state`` in place, after checking that the fused update can
+    continue it.  Raises ValueError for: another optimizer type (a param group whose keys are not those torch.optim.SGD
+    / Adam write, or state entries with other names); more than one param group, or another parameter
+    count; hyper-parameters other than lr that differ from ``opt`` (or dampening, amsgrad, maximize, decoupled weight
+    decay); Adam step counts that differ between parameters, or Adam state missing for some updated parameter; state
+    for a parameter the update never touches; a state tensor of the wrong shape.  Nothing is written unless every
+    check passes.  Returns (lr, step): step is the Adam step count, for SGD 1 when the dict carries state, else 0.  A
+    parameter without SGD momentum gets a zero buffer, which is what torch's first step does (its buffer = d)."""
+    groups = sd.get("param_groups") if isinstance(sd, dict) else None
+    if not isinstance(groups, (list, tuple)) or len(groups) != 1:
+        raise ValueError("the fused update runs one parameter group; the state_dict must have exactly one")
+    grp = groups[0]
+    n_params = len(list(model.parameters()))
+    if list(grp.get("params", ())) != list(range(n_params)):
+        raise ValueError(f"the param group lists {len(grp.get('params', ()))} parameters; the optimizer must be built "
+                         f"over all {n_params} of model.parameters()")
+    # the optimizer type: the group must carry exactly the keys torch.optim.SGD / Adam write (RMSprop, NAdam, RAdam,
+    # Adamax, ... share some of them, and SGD-like or Adam-like state names, but not the set), less the switches an
+    # older torch did not write yet
+    is_adam = isinstance(opt, Adam)
+    stock_keys = set(_stock_optimizer([torch.zeros(1)], opt).state_dict()["param_groups"][0])
+    extra, missing = set(grp) - stock_keys, stock_keys - set(grp) - set(_OPTIONAL_KEYS)
+    if extra or missing:
+        raise ValueError(f"state_dict of another optimizer type (param group keys {sorted(extra)} not written by, and "
+                         f"{sorted(missing)} missing from, torch.optim.{'Adam' if is_adam else 'SGD'}); this step runs "
+                         f"{type(opt).__name__}")
+    if is_adam:
+        want = {"betas": tuple(float(b) for b in opt.betas), "eps": float(opt.eps),
+                "weight_decay": float(opt.weight_decay), **_ADAM_FIXED}
+    else:
+        want = {"momentum": float(opt.momentum), "weight_decay": float(opt.weight_decay), **_SGD_FIXED}
+    for k, w in want.items():
+        got = grp.get(k, w if k in _OPTIONAL_KEYS and isinstance(w, bool) and not w else None)
+        try:
+            same = tuple(float(x) for x in got) == w if k == "betas" else \
+                (bool(got) == w if isinstance(w, bool) else float(got) == w)
+        except (TypeError, ValueError):
+            same = False
+        if not same:
+            raise ValueError(f"{k}={got!r} differs from the configuration the step was built with ({w!r})")
+    slots = {i: (p, off) for i, p, off in _updated_slots(model, active)}
+    keys = _state_keys(opt)
+    state = sd.get("state", {})
+    steps = set()
+    for i, entry in state.items():
+        if i not in slots:
+            raise ValueError(f"state for parameter {i}, which the fused update never touches (it gets no gradient)")
+        p = slots[i][0]
+        if set(entry) != set(keys) | ({"step"} if is_adam else set()):
+            raise ValueError(f"state[{i}] holds {sorted(entry)}; torch.optim.{'Adam' if is_adam else 'SGD'} keeps "
+                             f"{sorted(set(keys) | ({'step'} if is_adam else set()))}")
+        for k in keys:
+            t = entry.get(k)
+            if not torch.is_tensor(t) or tuple(t.shape) != tuple(p.shape):
+                raise ValueError(f"state[{i}][{k!r}] is not a tensor of shape {tuple(p.shape)}")
+        if is_adam:
+            steps.add(float(entry["step"]))
+    step = 1 if state else 0
+    if is_adam and state:
+        if len(steps) != 1 or len(state) != len(slots):
+            raise ValueError("the fused Adam update keeps one step count for every parameter it touches: the state "
+                             "must hold every one of them, with equal steps")
+        t = steps.pop()
+        if t < 1 or t != int(t):
+            raise ValueError(f"Adam step {t} is not a positive integer")
+        step = int(t)
+    for buf in flat_state.values():
+        buf.zero_()
+    for i, entry in state.items():
+        p, off = slots[i]
+        for k in keys:
+            flat_state[k][off:off + p.numel()].view_as(p).copy_(entry[k])
+    return float(grp["lr"]), step
+
+
 class TrainStep:
     """Options ``overlap_wgrad`` / ``parallel_branches`` put independent parts of the backward on forked streams
     inside the captured graph.  Forked sub-wave tensor-core GEMM nodes of one graph were found not to overlap under
@@ -117,7 +271,7 @@ class TrainStep:
                  use_graph: bool = True, process_group=None, seed: int = 0x5EED, double_buffer: bool = False,
                  overlap_wgrad: Optional[bool] = None, parallel_branches: bool = False,
                  overlap_allreduce: Optional[bool] = None, graph_collectives: Optional[bool] = None,
-                 optimizer: Optional[SGDNesterov] = None, mode: Optional[str] = None,
+                 optimizer: Optional[Optimizer] = None, mode: Optional[str] = None,
                  class_weight: Optional[torch.Tensor] = None, domain_weight: Sequence[float] = (1.0, 1.0),
                  allreduce: Optional[str] = None, mu: float = 0.0, sampler=None):
         """mode: 'legacy' (default) = the per-operator sequence (25 launches in one CUDA graph; the only mode that
@@ -145,7 +299,17 @@ class TrainStep:
         launch of every step (one launch more, in every mode, with or without the graph), each ``run()`` consumes one
         iteration of the sampler's current epoch (``start_epoch()``) and raises past its end, and ``load()`` /
         ``prefetch()`` / ``__call__`` raise.  Single rank only, and without ``double_buffer`` (nothing is left to
-        overlap)."""
+        overlap).
+
+        optimizer: ``SGDNesterov`` or ``Adam``, applied at the end of every ``run()`` (after the all-reduce).  Its state
+        is read and written in torch.optim's format by ``optimizer_state_dict()`` / ``load_optimizer_state_dict()``;
+        ``state_dict()`` / ``load_state_dict()`` add the dropout step counter, for a resume that continues the run."""
+        if optimizer is not None and not isinstance(optimizer, (SGDNesterov, Adam)):
+            raise TypeError(f"optimizer must be SGDNesterov or Adam, got {type(optimizer).__name__}")
+        if isinstance(optimizer, Adam):
+            b1, b2 = (float(b) for b in optimizer.betas)
+            if not (0.0 <= b1 < 1.0 and 0.0 <= b2 < 1.0) or not optimizer.eps > 0 or optimizer.weight_decay < 0:
+                raise ValueError(f"Adam needs 0 <= betas < 1, eps > 0, weight_decay >= 0: {optimizer}")
         if not model.training:
             raise ValueError("TrainStep needs model.train() (dropout state is fixed at construction)")
         if sampler is not None:
@@ -257,15 +421,23 @@ class TrainStep:
         self.bucket_early = self.flat_grad[:self.early_numel]
         self.bucket_late = self.flat_grad[self.early_numel:]
 
-        # optimizer state (SURVEY 8f n2): momentum buffers, device-resident learning rate, {norm, coef} stats
+        # optimizer state (SURVEY 8f n2): momentum buffers (SGD) or the two moments and the step count (Adam),
+        # device-resident learning rate, {norm, coef} stats
         self.opt = optimizer
+        self._opt_stepped = False           # SGD: an update has run or been loaded (torch's state is empty before)
         if optimizer is not None:
-            self.momentum_buf = torch.zeros_like(self.flat_grad)
+            if isinstance(optimizer, Adam):
+                self.exp_avg = torch.zeros_like(self.flat_grad)
+                self.exp_avg_sq = torch.zeros_like(self.flat_grad)
+                self.adam_step = torch.zeros(1, device=dev, dtype=torch.int64)      # t, advanced by the kernel
+                ws_bytes = _lib.load().ta3n_adam_workspace_bytes()
+            else:
+                self.momentum_buf = torch.zeros_like(self.flat_grad)
+                ws_bytes = _lib.load().ta3n_sgd_workspace_bytes()
             self.lr_dev = torch.full((1,), float(optimizer.lr), device=dev, dtype=torch.float32)
-            self._lr_host = torch.full((1,), float(optimizer.lr), dtype=torch.float32).pin_memory()
             self.grad_stats = torch.zeros(2, device=dev, dtype=torch.float32)     # [total_norm, clip_coef]
-            self.opt_ws = torch.zeros(max(1, _lib.load().ta3n_sgd_workspace_bytes() // 4), device=dev,
-                                      dtype=torch.float32)
+            # zero-initialised: the Adam kernel's arrival counter starts (and stays, between launches) at 0
+            self.opt_ws = torch.zeros(max(1, ws_bytes // 4), device=dev, dtype=torch.float32)
             # parameters the configured losses never reach keep grad = None in the reference, and torch.optim.SGD then
             # leaves them alone (no weight decay, no momentum; main.py:83): mask their slots out of the fused update
             R = self.R
@@ -559,21 +731,76 @@ class TrainStep:
 
     # -- the fixed launch sequence ---------------------------------------------------------------------
     def _enqueue_optimizer(self):
-        """clip_grad_norm_ + SGD-Nesterov over the flat buffers (main.py:578-583): two launches."""
+        """clip_grad_norm_ + SGD-Nesterov or Adam over the flat buffers (main.py:578-583): two launches (one without
+        clipping)."""
         o = self.opt
         clip = float(o.clip_gradient) if o.clip_gradient is not None else 0.0
+        if isinstance(o, Adam):
+            check(_lib.load().ta3n_adam_step_masked(
+                _P(self.flat_param), _P(self.flat_grad), _P(self.exp_avg), _P(self.exp_avg_sq), self.flat_grad.numel(),
+                _P(self.lr_dev), _P(self.adam_step), float(o.betas[0]), float(o.betas[1]), float(o.eps),
+                float(o.weight_decay), clip, _P(self.opt_ws), self.opt_ws.numel() * 4, _P(self.grad_stats),
+                _P(self.active_mask), TF._stream()))
+            return
         check(_lib.load().ta3n_sgd_nesterov_step_masked(
             _P(self.flat_param), _P(self.flat_grad), _P(self.momentum_buf), self.flat_grad.numel(),
             _P(self.lr_dev), float(o.momentum), float(o.weight_decay), clip, _P(self.opt_ws),
             self.opt_ws.numel() * 4, _P(self.grad_stats), _P(self.active_mask), TF._stream()))
 
     def set_lr(self, lr: float):
-        """Per-step learning-rate schedules (main.py:800-802): one 4-byte async copy, no re-capture."""
+        """Per-step learning-rate schedules (main.py:800-802): one 4-byte fill on the stream, no re-capture."""
         if self.opt is None:
-            raise ValueError("set_lr needs TrainStep(optimizer=SGDNesterov(...))")
-        self._lr_host[0] = float(lr)
-        self.lr_dev.copy_(self._lr_host, non_blocking=True)
+            raise ValueError("set_lr needs TrainStep(optimizer=SGDNesterov(...) or Adam(...))")
+        # the value travels in the launch itself: a pinned staging buffer rewritten every step can be read by a copy
+        # still queued behind earlier steps, which would apply a later step's rate
+        self.lr_dev.fill_(float(lr))
         self.opt.lr = float(lr)
+
+    # -- checkpoints ------------------------------------------------------------------------------------------------
+    def _flat_state(self):
+        return {k: getattr(self, "momentum_buf" if k == "momentum_buffer" else k) for k in _state_keys(self.opt)}
+
+    def optimizer_state_dict(self) -> dict:
+        """The optimizer's state in torch.optim's format: what ``torch.optim.SGD`` / ``Adam(model.parameters(), ...)``
+        (main.py:83 / 86) would return from ``state_dict()`` at this point of training, so main.py's checkpoint
+        (``'optimizer': optimizer.state_dict()``, main.py:266-274) keeps its format.  Synchronises with the device."""
+        if self.opt is None:
+            raise ValueError("optimizer_state_dict needs TrainStep(optimizer=...)")
+        step = int(self.adam_step.item()) if isinstance(self.opt, Adam) else int(self._opt_stepped)
+        return optimizer_state_to_torch(self.model, self.opt, self._flat_state(), self.active_mask, step)
+
+    def load_optimizer_state_dict(self, sd: dict) -> None:
+        """Continue from a torch.optim ``state_dict()`` -- this class's, or a stock SGD / Adam's built over
+        ``model.parameters()`` (main.py:102-104, --resume_hp).  The state is copied into the flat buffers in place, so
+        the captured graph stays valid; the learning rate and Adam's step count are set from the dict.  Raises
+        ValueError when the update cannot continue it (``optimizer_state_from_torch``)."""
+        if self.opt is None:
+            raise ValueError("load_optimizer_state_dict needs TrainStep(optimizer=...)")
+        lr, step = optimizer_state_from_torch(self.model, self.opt, sd, self._flat_state(), self.active_mask)
+        self.set_lr(lr)
+        if isinstance(self.opt, Adam):
+            self.adam_step.fill_(step)
+        self._opt_stepped = step > 0
+
+    def state_dict(self) -> dict:
+        """``{'optimizer': optimizer_state_dict() (None without an optimizer), 'step_counter': int}``.  The step counter
+        keys the dropout masks, so a run resumed from it draws the masks the uninterrupted run would have drawn."""
+        return {"optimizer": None if self.opt is None else self.optimizer_state_dict(),
+                "step_counter": int(self.step_counter.item())}
+
+    def load_state_dict(self, sd: dict) -> None:
+        """Resume from ``state_dict()``: the optimizer state (in place, no re-capture) and the dropout step counter.
+        With the library's peer all-reduce the counter is also the all-reduce's sequence number, which must only grow:
+        a counter below the current one is refused there."""
+        counter = int(sd["step_counter"])
+        if (sd.get("optimizer") is None) != (self.opt is None):
+            raise ValueError("the state_dict and this TrainStep disagree on whether there is an optimizer")
+        if self.ar is not None and counter < int(self.step_counter.item()):
+            raise ValueError(f"step_counter {counter} is below the current {int(self.step_counter.item())}: the peer "
+                             "all-reduce needs an increasing sequence number; load into a freshly built TrainStep")
+        if self.opt is not None:
+            self.load_optimizer_state_dict(sd["optimizer"])
+        self.step_counter.fill_(counter)
 
     def _enqueue(self, at_split=None, optimizer=False):
         """Enqueue the whole step on the current stream.  ``at_split()`` (optional) is called at the point
@@ -834,6 +1061,7 @@ class TrainStep:
                 self._allreduce(self.flat_grad)
         if not opt_done:
             self._enqueue_optimizer()             # after the all-reduce: every rank applies the same update
+        self._opt_stepped = self._opt_stepped or self.opt is not None
         self.install_grads()
         return self.loss
 
