@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define TA3N_ABI_VERSION 6
+#define TA3N_ABI_VERSION 7
 
 enum {
   TA3N_OK = 0,
@@ -334,6 +334,53 @@ int ta3n_eval_head(const float* feat_video, int rows, int H, int C, const float*
                    const int* k_host, const float* attn, int R, long long attn_ld, float* logits,
                    ta3n_eval_accum* accum, long long* confusion, float* scores, float* attn_out, long long n_epoch,
                    void* workspace, size_t workspace_bytes, ta3n_stream_t stream);
+
+/* ---- training meters (main.py:309-617 train(): losses, losses_c/_a/_e/_s, top1, top5) ------------------------- */
+/* Epoch accumulator in device memory (8-byte aligned; zero it to start an epoch).  Meters, in this order:
+ * 0 loss, 1 loss_c, 2 loss_a, 3 loss_e, 4 loss_s; AverageMeter.update(val, n) (main.py:772-787) is
+ * sum += val * n, count += n, val = val, except that a step giving a meter n = 0 sets val and leaves sum.           */
+typedef struct {
+  double sum[5];              /* sum over steps of val * n                                                          */
+  double val[5];              /* the last step's val (0 until a step updates the meter)                             */
+  long long count[5];         /* sum over steps of n (0 for a meter whose term is switched off)                      */
+  long long correct[4];       /* real source rows whose label ranks below k[i], over the epoch                       */
+  long long correct_step[4];  /* the same for the last step                                                          */
+  long long rows;             /* real source rows over the epoch (the n of top1 / top5)                              */
+  long long rows_step;        /* real source rows of the last step                                                   */
+  long long steps;            /* launches folded in so far                                                           */
+  unsigned int arrive;        /* arrival counter of the launch, 0 between launches                                   */
+  unsigned int pad_;
+} ta3n_train_stats;
+
+size_t ta3n_train_stats_workspace_bytes(int M);
+/* One launch per training step, after the step's loss launches: it reads the logits the loss kernels read and folds
+ * the meters main.py keeps (main.py:446-571) into *accum.  Inputs as for ta3n_loss_fwd_bwd (M = Bs + Bt rows, source
+ * first; valid_rows {real source rows vs, real target rows vt} or NULL = {Bs, Bt}); pred_video's target rows are the
+ * logits the attentive entropy reads (under MCD: those of the reverse pass).  Per step, with rows past vs / vt
+ * ignored:
+ *   loss    val = *loss as written (the value backpropagated), n = 1;
+ *   loss_c  val = sum w_y ce / sum w_y over the real source rows (w_y = class_weight[y], NULL: 1), plus the same
+ *           for pred2_s (the second classifier, MCD); n = vs;
+ *   loss_a  val = sum over the levels on in flags (1 relation, 2 video, 4 frame) of the domain CE of
+ *           CrossEntropyLoss(weight = domain_weight) over the level's real rows (labels 0 source, 1 target);
+ *           n = rows of the LAST level on in the order relation, video, frame: (vs+vt)*R, vs+vt, (vs+vt)*T;
+ *   loss_e  (flags & 8) val = mean over the vs+vt real rows of (1 + H(softmax(pred_dom))) * H(softmax(pred_video)),
+ *           without gamma; n = vt;
+ *   loss_s  (MCD: pred2_s non-NULL, and pred2_t when Bt > 0) val = -mean over the vt real target rows and C classes of
+ *           |softmax(pred_video[Bs + r]) - softmax(pred2_t[r])|, 0 when vt = 0; n = vt;
+ *   top-k   correct@k over the real source rows of pred_video; TIES RANK BY CLASS INDEX as in ta3n_eval_head:
+ *           rank = #{j : z_j > z_y} + #{j < y : z_j == z_y}, correct@k = rank < k.
+ * A label outside [0, C) or a NaN among a row's logits makes that row's CE NaN (so loss_c's val) and the row counts
+ * at no k (it still counts in rows), as in ta3n_eval_head.  Row terms are computed in fp32 and summed in fp64; each CTA
+ * writes its partial sums (row order) to the workspace and the last CTA to arrive folds them in CTA order into *accum,
+ * advances accum->steps and re-arms accum->arrive: reruns are bit-identical (no float atomics).  Nothing the step reads
+ * is written.  n_k in [1, 4], k_host[i] in [1, C]; flags in [0, 15].  Kernel label "train_stats".                    */
+int ta3n_train_stats_accumulate(const float* pred_video, const long long* labels, const float* pred_rel,
+                                const float* pred_dom_video, const float* pred_frame, const float* pred2_s,
+                                const float* pred2_t, const float* loss, int Bs, int Bt, int T, int R, int C,
+                                int flags, const int* valid_rows, const float* class_weight,
+                                const float* domain_weight_host, int n_k, const int* k_host, ta3n_train_stats* accum,
+                                void* workspace, size_t workspace_bytes, ta3n_stream_t stream);
 
 /* ---- the training step as one step program (SURVEY 8a rows a1-a13 + 8f row n1) ----------------------------- */
 /* main.py:418 (model forward, models.py:545-722 trn-m branch), main.py:446, 508-538, 559-562 (composed loss:

@@ -11,7 +11,7 @@ import threading
 
 from . import build as _build
 
-ABI_VERSION = 6     # TA3N_ABI_VERSION of include/ta3n_b200.h that SIGNATURES mirrors
+ABI_VERSION = 7     # TA3N_ABI_VERSION of include/ta3n_b200.h that SIGNATURES mirrors
 
 TA3N_GEMM_FP32_SIMT = 0
 TA3N_GEMM_TF32_TCGEN05 = 1
@@ -111,6 +111,9 @@ SIGNATURES = {
     "ta3n_eval_workspace_bytes": (_SZ, [_I]),
     "ta3n_eval_head": (_I, [_VP, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _I, _IP, _VP, _I, C.c_longlong, _VP,
                             _VP, _VP, _VP, _VP, C.c_longlong, _VP, _SZ, _VP]),
+    "ta3n_train_stats_workspace_bytes": (_SZ, [_I]),
+    "ta3n_train_stats_accumulate": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP, _VP,
+                                         C.POINTER(C.c_float), _I, _IP, _VP, _VP, _SZ, _VP]),
     "ta3n_step_workspace_bytes": (_SZ, [C.POINTER(StepDesc)]),
     "ta3n_step_run_phased": (_I, [C.POINTER(StepDesc), _VP]),
     "ta3n_allreduce_flag_bytes": (_SZ, [_I]),

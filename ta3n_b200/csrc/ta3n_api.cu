@@ -10,6 +10,7 @@
 #include "allreduce.cuh"
 #include "gather.cuh"
 #include "eval.cuh"
+#include "train_stats.cuh"
 
 #include <functional>
 
@@ -1086,6 +1087,54 @@ int ta3n_eval_head(const float* feat_video, int rows, int H, int C, const float*
   pre_launch("eval_head", S(stream));
   launch_kernel(eval_head_kernel, grid, kEvalThreads, smem, S(stream), a,
                 reinterpret_cast<EvalPartial*>(workspace));
+  return after_launch();
+}
+
+// ------------------------------------------------------------------------------------------------
+// training meters (include/ta3n_b200.h: ta3n_train_stats_accumulate)
+// ------------------------------------------------------------------------------------------------
+static int train_stats_grid(int M) { return (M + kStatsRows - 1) / kStatsRows; }
+
+size_t ta3n_train_stats_workspace_bytes(int M) {
+  return M < 1 ? 0 : Arena::round((size_t)train_stats_grid(M) * sizeof(TrainStatsPartial));
+}
+
+int ta3n_train_stats_accumulate(const float* pred_video, const long long* labels, const float* pred_rel,
+                                const float* pred_dom_video, const float* pred_frame, const float* pred2_s,
+                                const float* pred2_t, const float* loss, int Bs, int Bt, int T, int R, int C,
+                                int flags, const int* valid_rows, const float* class_weight,
+                                const float* domain_weight_host, int n_k, const int* k_host, ta3n_train_stats* accum,
+                                void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
+  TA3N_REQUIRE(accum != nullptr, "null accumulator");
+  TA3N_REQUIRE(reinterpret_cast<uintptr_t>(accum) % 8 == 0, "accum must be 8-byte aligned");
+  TA3N_REQUIRE(Bs >= 1 && Bt >= 0 && T >= 1 && R >= 1 && C >= 1, "bad sizes (M = Bs + Bt must be >= 1, Bs >= 1)");
+  TA3N_REQUIRE((long long)Bs + Bt <= INT32_MAX - kStatsRows, "too many rows");
+  TA3N_REQUIRE(flags >= 0 && flags <= 15, "flags must be a combination of 1, 2, 4 and 8");
+  TA3N_REQUIRE(n_k >= 1 && n_k <= kEvalMaxK && k_host, "between 1 and 4 top-k values");
+  for (int i = 0; i < n_k; ++i)
+    if (k_host[i] < 1 || k_host[i] > C)
+      return fail(TA3N_ERR_INVALID, "ta3n_train_stats_accumulate: top-k value %d is outside [1, C=%d]", k_host[i], C);
+  TA3N_REQUIRE(pred_video && labels && pred_rel && pred_dom_video && pred_frame && loss, "null input");
+  TA3N_REQUIRE(pred2_s || !pred2_t, "pred2_t without pred2_s (MCD needs both)");
+  TA3N_REQUIRE(!pred2_s || pred2_t || Bt == 0, "pred2_s without pred2_t (MCD needs both when Bt > 0)");
+  TA3N_REQUIRE(domain_weight_host != nullptr, "null domain_weight_host");
+  const int M = Bs + Bt;
+  const int grid = train_stats_grid(M);
+  const size_t need = ta3n_train_stats_workspace_bytes(M);
+  TA3N_REQUIRE(workspace && reinterpret_cast<uintptr_t>(workspace) % 16 == 0, "null or misaligned workspace");
+  if (workspace_bytes < need)
+    return fail(TA3N_ERR_WORKSPACE, "ta3n_train_stats_accumulate: workspace too small (%zu < %zu bytes)",
+                workspace_bytes, need);
+  TrainStatsArgs a;
+  a.pred_video = pred_video, a.labels = labels, a.pred_rel = pred_rel, a.pred_dom = pred_dom_video;
+  a.pred_frame = pred_frame, a.pred2_s = pred2_s, a.pred2_t = pred2_t, a.loss = loss, a.valid_rows = valid_rows;
+  a.class_weight = class_weight, a.accum = accum;
+  a.dw[0] = domain_weight_host[0], a.dw[1] = domain_weight_host[1];
+  a.Bs = Bs, a.Bt = Bt, a.T = T, a.R = R, a.C = C, a.flags = flags, a.n_k = n_k;
+  for (int i = 0; i < kEvalMaxK; ++i) a.k[i] = i < n_k ? k_host[i] : 0;
+  pre_launch("train_stats", S(stream));
+  launch_kernel(train_stats_kernel, grid, kStatsThreads, 0, S(stream), a,
+                reinterpret_cast<TrainStatsPartial*>(workspace));
   return after_launch();
 }
 

@@ -27,6 +27,7 @@ import math
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -66,6 +67,80 @@ class Adam:
 
 
 Optimizer = Union[SGDNesterov, Adam]
+
+_STATS_WORDS = 27       # int64 words of ta3n_train_stats (216 bytes)
+_METERS = ("loss", "loss_c", "loss_a", "loss_e", "loss_s")
+
+
+@dataclass
+class Meter:
+    """One ``AverageMeter`` of main.py:772-787: the last step's ``val``, ``sum`` of val * n, ``count`` = sum of n and
+    ``avg`` = sum / count (0 while count is 0, as a fresh AverageMeter)."""
+    val: float = 0.0
+    avg: float = 0.0
+    sum: float = 0.0
+    count: int = 0
+
+
+@dataclass
+class TrainStats:
+    """The meters of main.py's train() (main.py:311-320) over the steps since the last ``reset_stats()``: ``loss``,
+    ``loss_c``, ``loss_a``, ``loss_e``, ``loss_s`` and, per k of ``topk``, the precision meter ``prec[k]`` (percent;
+    ``top1`` / ``top5`` when those k are kept).  A meter whose term is switched off keeps count 0.  ``correct`` and
+    ``rows``: the epoch's top-k hits and real source rows; ``steps``: the steps folded in."""
+    loss: Meter
+    loss_c: Meter
+    loss_a: Meter
+    loss_e: Meter
+    loss_s: Meter
+    prec: Dict[int, Meter]
+    topk: Tuple[int, ...]
+    correct: Tuple[int, ...]
+    rows: int
+    steps: int
+
+    @property
+    def top1(self) -> Optional[Meter]:
+        return self.prec.get(1)
+
+    @property
+    def top5(self) -> Optional[Meter]:
+        return self.prec.get(5)
+
+
+def parse_train_stats(words, topk: Sequence[int]) -> TrainStats:
+    """A ``ta3n_train_stats`` accumulator (its 27 int64 words, host memory) as ``TrainStats``."""
+    w = np.asarray(words, dtype=np.int64)
+    sums, vals = w[0:5].view(np.float64), w[5:10].view(np.float64)
+    counts, correct, step = w[10:15], w[15:19], w[19:23]
+    rows, rows_step, steps = int(w[23]), int(w[24]), int(w[25])
+    meters = {}
+    for i, name in enumerate(_METERS):
+        n = int(counts[i])
+        meters[name] = Meter(val=float(vals[i]), avg=float(sums[i]) / n if n else 0.0, sum=float(sums[i]), count=n)
+    prec = {}
+    for q, k in enumerate(topk):
+        # accuracy() gives 100 * correct / batch (main.py:821) and top1.update(prec1, batch): sum = 100 * correct
+        val = 100.0 * int(step[q]) / rows_step if rows_step else 0.0
+        total = 100.0 * int(correct[q])
+        prec[int(k)] = Meter(val=val if steps else 0.0, avg=total / rows if rows else 0.0, sum=total, count=rows)
+    return TrainStats(prec=prec, topk=tuple(int(k) for k in topk), correct=tuple(int(c) for c in correct[:len(topk)]),
+                      rows=rows, steps=steps, **meters)
+
+
+class TrainStatsSnapshot:
+    """``TrainStep.stats_async()``: the accumulator copied to pinned host memory behind an event."""
+
+    def __init__(self, host: torch.Tensor, event, topk: Tuple[int, ...]):
+        self._host, self._event, self._topk = host, event, topk
+
+    def done(self) -> bool:
+        return self._event.query()
+
+    def result(self) -> TrainStats:
+        """Wait for the copy (not for later work on the stream) and return the snapshot."""
+        self._event.synchronize()
+        return parse_train_stats(self._host.numpy(), self._topk)
 
 
 def lr_dann(lr0: float, p: float) -> float:
@@ -273,7 +348,8 @@ class TrainStep:
                  overlap_allreduce: Optional[bool] = None, graph_collectives: Optional[bool] = None,
                  optimizer: Optional[Optimizer] = None, mode: Optional[str] = None,
                  class_weight: Optional[torch.Tensor] = None, domain_weight: Sequence[float] = (1.0, 1.0),
-                 allreduce: Optional[str] = None, mu: float = 0.0, sampler=None):
+                 allreduce: Optional[str] = None, mu: float = 0.0, sampler=None, stats: bool = False,
+                 stats_topk: Sequence[int] = (1, 5)):
         """mode: 'legacy' (default) = the per-operator sequence (25 launches in one CUDA graph; the only mode that
         supports use_attn_frame); 'phased' = the step program as 14 launches (ta3n_step_run_phased; default when class /
         domain weights or a scheduled beta are given).  class_weight / domain_weight: the weights of criterion /
@@ -303,7 +379,12 @@ class TrainStep:
 
         optimizer: ``SGDNesterov`` or ``Adam``, applied at the end of every ``run()`` (after the all-reduce).  Its state
         is read and written in torch.optim's format by ``optimizer_state_dict()`` / ``load_optimizer_state_dict()``;
-        ``state_dict()`` / ``load_state_dict()`` add the dropout step counter, for a resume that continues the run."""
+        ``state_dict()`` / ``load_state_dict()`` add the dropout step counter, for a resume that continues the run.
+
+        stats: keep the meters of main.py's train() on the device (``ta3n_train_stats_accumulate``, one launch per
+        step after the loss launches, in the same graph): the loss, each loss term and the top-k accuracy of
+        ``stats_topk`` (one to four k in [1, C]) on the batch's real source rows.  ``stats()`` reads them back,
+        ``stats_async()`` without stalling the stream, ``reset_stats()`` starts an epoch.  Single rank only."""
         if optimizer is not None and not isinstance(optimizer, (SGDNesterov, Adam)):
             raise TypeError(f"optimizer must be SGDNesterov or Adam, got {type(optimizer).__name__}")
         if isinstance(optimizer, Adam):
@@ -321,6 +402,10 @@ class TrainStep:
                                           "PairedFeatureLoader + load() / prefetch()")
             if (int(sampler.batch[0]), int(sampler.batch[1])) != (int(batch_source), int(batch_target)):
                 raise ValueError(f"sampler batches {sampler.batch} != TrainStep({batch_source}, {batch_target})")
+        if stats and (dist.get_world_size(process_group) if dist.is_initialized() else 1) > 1:
+            # each rank would fold its own shard; the global meters need the per-level sums combined every step
+            raise NotImplementedError("stats=True keeps the meters of a single rank; with several ranks they would "
+                                      "have to be combined across ranks every step")
         self.sampler = sampler
         ens = getattr(model, "ens_DA", "none")
         if model.use_attn == "general" or ens not in ("none", "MCD") or model.frame_aggregation != "trn-m":
@@ -497,6 +582,7 @@ class TrainStep:
             drop_v=TF.DropSpec(p=dv, seed=seed ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec())
         if self.mcd:
             self._init_mcd(seed, di, dv, offs)
+        self._init_stats(stats, stats_topk)
         self.outputs = None
         self.branch_stream = torch.cuda.Stream(device=dev) if parallel_branches else None
         self.overlap_wgrad = bool(overlap_wgrad)
@@ -521,6 +607,72 @@ class TrainStep:
             self.xs, self.xt, self.labels, self.valid = self.slots[0]
         if sampler is not None:
             sampler.rewind()        # the capture's warm-up ran one gather
+        if self.keep_stats:
+            self.reset_stats()      # and folded one step into the meters
+
+    def _init_stats(self, stats, topk):
+        """The meters' accumulator (ta3n_train_stats), its workspace and the launch's host arguments."""
+        self.keep_stats = bool(stats)
+        if not self.keep_stats:
+            return
+        self.stats_topk = tuple(int(k) for k in topk)
+        if not 1 <= len(self.stats_topk) <= 4 or any(not 1 <= k <= self.C for k in self.stats_topk):
+            raise ValueError(f"stats_topk {self.stats_topk}: between one and four values in [1, C={self.C}]")
+        lib = _lib.load()
+        self.stats_acc = torch.zeros(_STATS_WORDS, device=self.device, dtype=torch.int64)
+        self.stats_ws = torch.zeros(max(256, lib.ta3n_train_stats_workspace_bytes(self.M)), device=self.device,
+                                    dtype=torch.uint8)
+        self._stats_k = (C.c_int * len(self.stats_topk))(*self.stats_topk)
+        # the launch forks off the step's stream and joins it at the end of the step, so that it runs beside the
+        # backward / the optimizer instead of in front of them (nothing after the loss writes what it reads); a step
+        # split in two graphs keeps it on the stream (a branch may not join across graphs)
+        self.stats_stream = torch.cuda.Stream(device=self.device) if not self.split else None
+        # the per-operator sequence's loss kernel has no domain weights (the step program applies them)
+        self._stats_dw = (C.c_float * 2)(*(self.domain_weight if self.mode != "legacy" else (1.0, 1.0)))
+
+    def _enqueue_stats(self, lib, st, pred_video, pred_rel, pred_dom, pred_frame):
+        """The meters of this step (after the loss launches; reads logits and the loss, writes the accumulator), on
+        the forked stats stream when there is one (``_join_stats`` ends the branch)."""
+        p2s, p2t = (self.pred2_s, self.pred2_t) if self.mcd else (None, None)
+        if self.stats_stream is not None:
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream())
+            self.stats_stream.wait_event(ev)
+            st = self.stats_stream.cuda_stream
+        check(lib.ta3n_train_stats_accumulate(
+            _P(pred_video), _P(self.labels), _P(pred_rel), _P(pred_dom), _P(pred_frame), _P(p2s), _P(p2t),
+            _P(self.loss), self.Bs, self.Bt, self.T, self.R, self.C, self.flags, _P(self.valid),
+            _P(self.class_weight), self._stats_dw, len(self.stats_topk), self._stats_k, _P(self.stats_acc),
+            _P(self.stats_ws), self.stats_ws.numel(), st))
+
+    def _join_stats(self):
+        if self.keep_stats and self.stats_stream is not None:
+            torch.cuda.current_stream().wait_stream(self.stats_stream)
+
+    def _need_stats(self, what):
+        if not self.keep_stats:
+            raise ValueError(f"{what}() needs TrainStep(..., stats=True)")
+
+    def stats(self) -> TrainStats:
+        """The meters since the last ``reset_stats()`` (one blocking readback on the current stream)."""
+        self._need_stats("stats")
+        return parse_train_stats(self.stats_acc.cpu().numpy(), self.stats_topk)
+
+    def stats_async(self) -> TrainStatsSnapshot:
+        """Copy the meters into pinned host memory behind an event on the current stream and return at once;
+        ``.result()`` waits for that copy only.  Each call has its own host buffer."""
+        self._need_stats("stats_async")
+        host = torch.empty(_STATS_WORDS, dtype=torch.int64, pin_memory=True)
+        host.copy_(self.stats_acc, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        return TrainStatsSnapshot(host, ev, self.stats_topk)
+
+    def reset_stats(self) -> None:
+        """Start an epoch of meters (main.py builds fresh AverageMeters in every train() call): zeroes the accumulator
+        on the current stream, no re-capture."""
+        self._need_stats("reset_stats")
+        self.stats_acc.zero_()
 
     def _init_mcd(self, seed, di, dv, offs):
         """State of MCD's second pass: its dropout seeds, buffers, and a second gradient bucket with the bucket's
@@ -823,10 +975,14 @@ class TrainStep:
             self.sampler.enqueue_gather(self.xs, self.xt, self.labels, self.valid, st)     # this iteration's batch
         if self.mode != "legacy":
             check(lib.ta3n_step_run_phased(C.byref(self.step_descs[self.active][0]), st))
+            if self.keep_stats:
+                sb = self.step_bufs
+                self._enqueue_stats(lib, st, sb["pred_video"], sb["pred_rel"], sb["pred_dom"], sb["pred_frame"])
             if self.ar is not None:
                 self._enqueue_allreduce()         # same stream, same graph: step -> all-reduce -> optimizer
             if optimizer and self.opt is not None:
                 self._enqueue_optimizer()
+            self._join_stats()
             return
         check(lib.ta3n_counter_inc(_P(self.step_counter), st))          # fresh dropout masks per step
         saved, outputs, dims = TF.path_forward(self.spec, self.xs, self.xt, self.params, self.bufs, batch_gemms=True)
@@ -849,6 +1005,8 @@ class TrainStep:
             check(lib.ta3n_mcd_loss_fwd_bwd(_P(pred_video[self.Bs:]), _P(self.pred2_t), self.Bt, self.C, _P(self.valid),
                                             _P(self.loss), _P(self.g_video_t), _P(self.g_video2_t),
                                             _P(self.g_video[self.Bs:]), st))
+        if self.keep_stats:
+            self._enqueue_stats(lib, st, pred_video, pred_rel, pred_dom, pred_frame)
         gin = {"pred_video": self.g_video, "pred_rel": self.g_rel, "pred_dom_video": self.g_dom,
                "pred_frame": self.g_frame}
         # The data-gradient chain runs first; the weight-gradient GEMMs / bias sums it leaves behind are deferred
@@ -910,6 +1068,7 @@ class TrainStep:
             self._enqueue_allreduce()         # same stream, same graph: step -> all-reduce -> optimizer
         if optimizer and self.opt is not None:
             self._enqueue_optimizer()
+        self._join_stats()
 
     def _enqueue_with_collectives(self, optimizer=False):
         """The step with both gradient all-reduces issued in place (early bucket as soon as it is complete)."""
