@@ -108,7 +108,8 @@ def _check_tiles(what, got, ref, tol=X3_TOL):
     idx = [int(i) for i in torch.nonzero(ratio == ratio.max())[0]]
     assert worst <= 1.0, f"{what}: tile (plane, row, col) {idx} err {e.flatten()[ratio.argmax()].item():.3e} is " \
                          f"{worst:.2f}x its bound (normwise {err:.2e})"
-    print(f"[x3] {what}: normwise {err:.2e}, worst tile {worst:.3f} of its bound ({1 / worst:.1f}x headroom)")
+    headroom = f"{1 / worst:.1f}x headroom" if worst > 0 else "exact"
+    print(f"[x3] {what}: normwise {err:.2e}, worst tile {worst:.3f} of its bound ({headroom})")
     return worst
 
 
