@@ -1,29 +1,30 @@
 // gemm_wgmma.cuh -- Hopper (sm_90a) tensor-core engine for the segmented grouped GEMM.
 //
-// One CTA per 128 x 128 output tile, warp-specialised:
-//   warps 0..7 : two consumer warpgroups -- wgmma.mma_async m64n128k8 tf32, fp32 accumulators in registers (each
-//                warpgroup owns 64 rows of the tile), then the fused epilogue (apply_epilogue)
-//   warp 8     : TMA producer -- cp.async.bulk.tensor into a ring of 128B-swizzled stages (mbarrier handshake)
+// Both kernels compute 128 x 128 output tiles with 384 threads in three warpgroups:
+//   warps 0..7  : two consumer warpgroups -- wgmma.mma_async m64n128k8 tf32 with A from registers and B from shared
+//                 memory, fp32 accumulators in registers (each warpgroup owns 64 rows of the tile), then the fused
+//                 epilogue straight from the accumulator fragments
+//   warp 8      : TMA producer -- cp.async.bulk.tensor into a ring of 128B-swizzled stages (mbarrier handshake)
+//   warps 9..11 : B preparation -- write a K-major copy of each landed B tile beside it when B is MN-major (and, in
+//                 the precise kernel, the tf32 lo part of B), then arrive on the stage's ready barrier
+// setmaxnreg gives the producer warpgroup 40 registers per thread and the consumers 232.
 // Operands stay fp32 in HBM: the tf32 MMA reads the fp32 bit patterns (10-bit mantissa, fp32 range), so there is no
 // conversion pass and no second copy of any tensor in global memory.
 // The "gather" of TRN frame tuples, the source/target split and the per-frame dgrad are all
 // expressed as TMA coordinates / tensor maps per K-segment: nothing is materialised.
 //
-// wgmma reads tf32 operands from shared memory in K-major order only:
+// Operand layouts in a stage:
 //   K-major  (A(m,k)=A[m*ld+k]) : one TMA box {32 k, 128 rows}, SWIZZLE_128B; descriptor SW128, SBO = 1024 B,
 //                                 +32 B per K=8 step.  Read by the tensor core as loaded.
-//   MN-major (A(m,k)=A[k*ld+m]) : four TMA boxes {32 m, 32 k}, SWIZZLE_128B (16 B chunk index ^= k & 7); the consumer
-//                                 warps transpose the stage in place into the K-major layout above before the MMAs.
-// After the K loop the accumulators pass through a row-major shared-memory tile (TC_ACC_LD floats per row), from
-// which every epilogue warp reads whole 32-column row pieces.
+//   MN-major (A(m,k)=A[k*ld+m]) : four TMA boxes {32 m, 32 k}, SWIZZLE_128B (16 B chunk index ^= k & 7).  wgmma reads
+//                                 shared-memory tf32 operands K-major only, so MN-major B is transposed by warps
+//                                 9..11; A, fed from registers, is read in whichever layout it landed.
 //
-// The precise forward kernel (seg_gemm_tc_x3_kernel, "tf32x3") adds a producer warpgroup: 384 threads, warp 8 for
-// TMA and warps 9..11 that write the tf32 lo tile of each landed B tile (transposing MN-major B on the way).  Its
-// consumers take A from registers: each thread loads its own fragment words from the raw stage and splits them
-// there, so the MMA warps do nothing but load, split and issue in the K loop.  setmaxnreg gives the producer
-// warpgroup 40 registers per thread and the consumers 232.  Its CTAs are persistent (one wave, a static task list per
-// CTA): the producer warps run ahead into the next task, and the epilogue works straight from the accumulator
-// registers.
+// The plain kernel (seg_gemm_tc_kernel, "tf32") runs one tile per CTA with one accumulator over its whole K range;
+// its TFLOAT32 tensor maps make the TMA unit round each operand to tf32.  The precise kernel (seg_gemm_tc_x3_kernel,
+// "tf32x3") splits both operands into hi + lo tf32 pieces (the consumers split their A fragments in registers) and
+// issues three products per K step; its CTAs are persistent (one wave, a static task list per CTA) and the producer
+// warps run ahead into the next task.
 #pragma once
 
 #include <cuda.h>
@@ -40,19 +41,24 @@
 namespace ta3n {
 
 constexpr int TC_BM = 128, TC_BN = 128, TC_BK = 32;
-constexpr int TC_THREADS = 288;        // warps 0..7: two consumer warpgroups; warp 8: TMA producer
+constexpr int TC_THREADS = 384;        // warps 0..7: two consumer warpgroups; warp 8: TMA producer; 9..11: B preparation
 constexpr int TC_CONSUMER_WARPS = 8;
+constexpr int TC_B_WARPS = 3;
+constexpr int TC_B_THREADS = 32 * TC_B_WARPS;
+// one CTA per SM: 65536 / 384 threads, rounded down to the allocation unit of 8, is 168 registers per thread at launch
+constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;
+static_assert(128 * TC_PRODUCER_REGS + 256 * TC_CONSUMER_REGS <= TC_THREADS * 168,
+              "setmaxnreg budget exceeds the registers of one CTA");
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 4;   // 16 KB
 constexpr int TC_B_BYTES = TC_BN * TC_BK * 4;   // 16 KB
 constexpr int TC_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;
-// 4 stages (129 KB, one CTA per SM): the grids of this workload are within a wave, so a CTA is alone on its SM and
-// bound by TMA latency -- the bytes in flight per CTA matter more than a second resident CTA.
+// 4 stages (one CTA per SM; 129 KB of ring, or 193 KB when the plain kernel keeps a K-major copy of MN-major B, as the
+// precise kernel always does): the grids of this workload are within a wave, so a CTA is alone on its SM and bound by
+// TMA latency -- the bytes in flight per CTA matter more than a second resident CTA.
 constexpr int TC_STAGES = 4;
-constexpr int tc_smem_bytes(int stages) { return stages * TC_STAGE_BYTES + 1024; }   // + 1024 B alignment slack
-// accumulator tile in shared memory: [128 rows][132 floats] (16 B aligned rows, conflict-free row-per-lane reads)
-constexpr int TC_ACC_LD = TC_BN + 4;
-constexpr int TC_ACC_BYTES = TC_BM * TC_ACC_LD * 4;
-static_assert(TC_ACC_BYTES <= TC_STAGES * TC_STAGE_BYTES, "the per-launch kernel reuses its operand ring");
+// the plain kernel's stage: [A | B] as loaded, + [B K-major] when B is MN-major
+__host__ __device__ constexpr int tc_stage_bytes(bool b_kmaj) { return TC_STAGE_BYTES + (b_kmaj ? 0 : TC_B_BYTES); }
+constexpr int tc_smem_bytes(bool b_kmaj) { return TC_STAGES * tc_stage_bytes(b_kmaj) + 1024; }   // + alignment slack
 #ifndef TA3N_MAX_MAPS
 #define TA3N_MAX_MAPS 64
 #endif
@@ -93,8 +99,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// the 256 consumer threads (warps 0..7) only
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
   asm volatile(
@@ -213,44 +217,41 @@ __device__ __forceinline__ void tc_prep_store(const uint32_t base, const int t, 
   for (int i = 0; i < 4; ++i)
     sts4(base + kmaj_chunk(4 * mq + i, kq), make_float4(f4_at(r[0], i), f4_at(r[1], i), f4_at(r[2], i), f4_at(r[3], i)));
 }
-// Make a landed stage readable by wgmma: MN-major operands transposed in place.  Called by all 256 consumer threads;
-// ends with the stage visible to the tensor core.
-__device__ __forceinline__ void tc_prep_stage(const uint32_t a_base, const uint32_t b_base, const bool a_kmaj,
-                                              const bool b_kmaj) {
-  if (a_kmaj && b_kmaj) return;
-  const int t = threadIdx.x;
-  float4 ra[4], rb[4];
-  if (!a_kmaj) tc_prep_load(a_base, t, ra);
-  if (!b_kmaj) tc_prep_load(b_base, t, rb);
-  consumer_sync();                                  // every read of the stage before the in-place transposed writes
-  if (!a_kmaj) tc_prep_store(a_base, t, ra);
-  if (!b_kmaj) tc_prep_store(b_base, t, rb);
-  fence_proxy_async();                              // generic-proxy writes -> the tensor core's reads
-  consumer_sync();
+// B preparation warps (thread t of 96): the MN-major B tile at b_mn, transposed into the K-major SW128 tile at b_k.
+__device__ __forceinline__ void tc_transpose_b(const uint32_t b_mn, const uint32_t b_k, const int t) {
+#pragma unroll 1
+  for (int blk = t; blk < 256; blk += TC_B_THREADS) {
+    float4 r[4];
+    tc_prep_load(b_mn, blk, r);
+    tc_prep_store(b_k, blk, r);
+  }
 }
 
-// accumulator fragments -> the row-major accumulator tile (consumer thread t)
-__device__ __forceinline__ void tc_store_acc(float* acc, const float (&d)[64], const int t) {
-  const int lane = t & 31;
-  const int row0 = (t >> 7) * 64 + ((t >> 5) & 3) * 16 + (lane >> 2);
-#pragma unroll
-  for (int j = 0; j < 16; ++j)
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-      *reinterpret_cast<float2*>(acc + (row0 + 8 * h) * TC_ACC_LD + 8 * j + 2 * (lane & 3)) =
-          make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+// Per-thread part of the A fragment addresses of rows m = r0 (and r0 + 8, MN-major), column k = tq: the word offset
+// in the landed tile, whose bits 4..6 are the SW128 chunk index.  Stage bases are 1024-B aligned, so tc_load_a reaches
+// every other column by an XOR on those bits plus a constant, with no per-column offsets kept in registers.
+template <bool A_KMAJ>
+__device__ __forceinline__ uint32_t tc_a_thread_off(const int m, const int tq) {
+  return A_KMAJ ? kmaj_chunk(m, 0) + 4u * tq : mnmaj_chunk(tq, m >> 2) + 4u * (m & 3);
 }
-// 32 consecutive accumulator columns of one row
-__device__ __forceinline__ void acc_ld_32(const float* acc, int row, int col0, float* v) {
-  const float* p = acc + row * TC_ACC_LD + col0;
+
+// Consumer thread: the A fragment words of one slab (4 k-steps x 4 words, see wgmma_tf32_rs) from the landed A tile,
+// in either layout.  K-major loads are conflict-free (the SW128 chunk index differs per row), MN-major ones 2-way.
+//   K-major  (m, k = 8 ks + 4 half + tq): (a_base + off0) ^ ((2 ks + half) << 4), + 1024 for row r0 + 8 (same m & 7)
+//   MN-major (m, k = 8 ks + 4 half + tq): (a_base + off_m) ^ (half << 6), + 128 (4 half + 8 ks) k-rows
+template <bool A_KMAJ>
+__device__ __forceinline__ void tc_load_a(const uint32_t a_base, const uint32_t off0, const uint32_t off1,
+                                          uint32_t (&a)[16]) {
+  const uint32_t p0 = a_base + off0, p1 = a_base + off1;
 #pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const float4 q = *reinterpret_cast<const float4*>(p + j);
-    v[j] = q.x;
-    v[j + 1] = q.y;
-    v[j + 2] = q.z;
-    v[j + 3] = q.w;
-  }
+  for (int ks = 0; ks < TC_BK / 8; ++ks)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint32_t row = j & 1, half = j >> 1;
+      const uint32_t addr = A_KMAJ ? (p0 ^ ((2u * ks + half) << 4)) + 1024u * row
+                                   : ((row ? p1 : p0) ^ (half << 6)) + 512u * half + 1024u * ks;
+      a[4 * ks + j] = __float_as_uint(lds1(addr));
+    }
 }
 
 // ---- one output tile, by warp role ---------------------------------------------------------------------
@@ -270,11 +271,6 @@ __device__ __forceinline__ void tc_pipe_init(TcShared* sh) {
   }
   fence_barrier_init();
 }
-
-// What a tile of a split-K group does with its accumulator:
-//   TILE_FINAL   : fused epilogue -> C                       (ksplit == 1)
-//   TILE_PARTIAL : raw accumulator -> partial[split]         (a separate reduce pass applies the epilogue)
-enum : int { TILE_FINAL = 0, TILE_PARTIAL = 1 };
 
 // TMA producer (ONE thread): the n_iter K slabs [c_begin, c_begin + n_iter) of tile (m0, n0) into the ring.
 // `slabs` = slabs this CTA has pushed so far (advanced by the caller).
@@ -334,84 +330,6 @@ __device__ __forceinline__ void tc_produce(const TileCtx& ctx, const CUtensorMap
   }
 }
 
-// Consumer warpgroups (all 256 threads of warps 0..7): the n_iter slabs of the tile into d (warpgroup wg: rows
-// 64 wg .. 64 wg + 63).  One group of MMAs stays in flight while the next stage is prepared.
-template <int STAGES>
-__device__ __forceinline__ void tc_consume(const bool a_kmaj, const bool b_kmaj, const int n_iter, uint8_t* smem,
-                                           TcShared* sh, float (&d)[64]) {
-  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
-#pragma unroll
-  for (int j = 0; j < 64; ++j) d[j] = 0.f;
-  int prev = -1;
-  for (int it = 0; it < n_iter; ++it) {
-    const uint32_t gl = (uint32_t)it;
-    const int stage = (int)(gl % STAGES);
-    mbar_wait(&sh->full_bar[stage], (gl / STAGES) & 1u);
-    const uint32_t a_base = smem_u32(smem + stage * TC_STAGE_BYTES);
-    const uint32_t b_base = a_base + TC_A_BYTES;
-    tc_prep_stage(a_base, b_base, a_kmaj, b_kmaj);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < TC_BK / 8; ++ks) wgmma_tf32(d, wgmma_desc(a_base + wg * 64 * 128, ks), wgmma_desc(b_base, ks));
-    wgmma_commit();
-    wgmma_wait<1>();                    // the previous stage's MMAs are done: release it
-    if (prev >= 0) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sh->empty_bar[prev]);
-    }
-    prev = stage;
-  }
-  wgmma_wait<0>();
-  if (prev >= 0) {
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&sh->empty_bar[prev]);
-  }
-}
-
-// Epilogue (kEpiWarps warps; `ew` = this warp's index among them, 0-based).  Lane i of a warp owns accumulator row
-// 32*lq + i; it reads 32 consecutive columns of the accumulator tile `acc`, finishes them (fused epilogue) and writes
-// them as 8 x 16 B stores: every 128 B line of C is written whole.  The caller has synchronised after filling `acc`.
-template <int kEpiWarps>
-__device__ __forceinline__ void tc_epilogue(const TileCtx& ctx, const int m0, const int n0, const int split,
-                                            const int n_iter, const int mode, const float* acc, const int ew) {
-  const int lane = threadIdx.x & 31;
-  const int lq = ew & 3;                // row quarter of the tile
-  const Group e = ctx.g;                // register copy: no reloads behind the global stores
-  const int m = m0 + lq * 32 + lane;
-  const bool split_out = mode == TILE_PARTIAL;
-  float* const obase = split_out ? e.partial + (size_t)split * e.M * e.N : e.C;
-  const int ldo = split_out ? e.N : e.ldc;
-  constexpr int kColChunks = (TC_BN / 32) * 4 / kEpiWarps;      // column chunks of 32 per warp: 4 or 2
-  const int c0 = (ew / 4) * kColChunks;
-#pragma unroll 1
-  for (int c = c0; c < c0 + kColChunks; ++c) {
-    float v[32];
-    if (n_iter > 0) {
-      acc_ld_32(acc, lq * 32 + lane, c * 32, v);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = 0.f;
-    }
-    const int nb = n0 + c * 32;
-    if (m < e.M && nb < e.N) {
-      float* orow = obase + (size_t)m * ldo + nb;
-      const int nvalid = min(32, e.N - nb);
-      if (!split_out) {
-        TA3N_EPI_DISPATCH(e.flags, { epilogue_row32<EPI_F>(e, m, nb, nvalid, v); })
-      }
-      if (nb + 32 <= e.N && ((reinterpret_cast<uintptr_t>(orow) & 15u) == 0)) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(orow + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (nb + j < e.N) orow[j] = v[j];
-      }
-    }
-  }
-}
-
 // chunk range [c_begin, c_begin + n_iter) of split `split` of the group staged in ctx
 __device__ __forceinline__ void tc_chunk_range(const TileCtx& ctx, int split, int* c_begin, int* n_iter) {
   const Group& g = ctx.g;
@@ -422,8 +340,7 @@ __device__ __forceinline__ void tc_chunk_range(const TileCtx& ctx, int split, in
   *n_iter = max(0, min(total_chunks, *c_begin + cps) - *c_begin);
 }
 
-// ---- the per-launch kernel: one tile per CTA ---------------------------------------------------------
-// tile -> (group, split, m0, n0), shared by both per-launch kernels
+// linear tile number -> (split, m0, n0) within the group staged in ctx
 __device__ __forceinline__ void tc_decode(const TileCtx& ctx, const int tile, int* split, int* m0, int* n0) {
   const Group& g = ctx.g;
   int local = tile - g.tile_begin;
@@ -434,12 +351,152 @@ __device__ __forceinline__ void tc_decode(const TileCtx& ctx, const int tile, in
   *n0 = (local % g.tiles_n) * TC_BN;
 }
 
+// ---- epilogue straight from the accumulator fragment (consumer thread) ------------------------------------------
+// Thread (warp w, lane l) holds rows r0 = 64 (w / 4) + 16 (w % 4) + l / 4 and r0 + 8 of the tile, columns
+// 8j + 2(l % 4) + {0, 1} (see wgmma_tf32): v[4j + 2h + e] = (row r0 + 8h, column c0 + 8j + e), c0 = 2(l % 4).  A warp
+// store instruction then covers 8 rows x 32 B, whole sectors.
+__device__ __forceinline__ void frag_st2(float* p, const float x0, const float x1, const bool vec, const bool two) {
+  if (vec) {
+    *reinterpret_cast<float2*>(p) = make_float2(x0, x1);
+  } else {
+    p[0] = x0;
+    if (two) p[1] = x1;
+  }
+}
+
+// The fused epilogue of the fragment -> C.  The forward flag sets (bias, ReLU, RNG dropout) work from register copies
+// of the group fields and draw one rng_hash4 per 4-column group; every other set applies epilogue_t per element.
+template <int F>
+__device__ __forceinline__ void frag_epilogue(const Group& g, const int m0, const int n0, const float (&v)[64]) {
+  constexpr bool kFwd = F >= 0 && (F & ~(EPI_BIAS | EPI_RELU | EPI_DROP_RNG)) == 0;
+  const int M = g.M, N = g.N, ldc = g.ldc;
+  float* const C = g.C;
+  const bool vec = (N % 2) == 0 && (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) & 7u) == 0;
+  const float alpha = kFwd ? (g.alpha_dev ? g.alpha * __ldg(g.alpha_dev) : g.alpha) : 0.f;
+  const float* const bias = g.bias;
+  const uint64_t seed = g.seed, roff = g.rng_offset;
+  const uint64_t step = (kFwd && (F & EPI_DROP_RNG) && g.step_dev) ? *g.step_dev : 0ull;
+  const float dscale = g.drop_scale, dp = g.drop_p;
+  const uint32_t thr = rng_threshold(dp);
+  float b0[16], b1[16];                 // bias of the thread's columns, loaded before the first store
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int n = n0 + 8 * j;
+    b0[j] = kFwd && (F & EPI_BIAS) && n < N ? bias[n] : 0.f;
+    b1[j] = kFwd && (F & EPI_BIAS) && n + 1 < N ? bias[n + 1] : 0.f;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = m0 + 8 * h;
+    if (m >= M) continue;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int n = n0 + 8 * j;
+      if (n >= N) continue;
+      const bool two = n + 1 < N;
+      float x0 = v[4 * j + 2 * h], x1 = v[4 * j + 2 * h + 1];
+      if (kFwd) {
+        x0 *= alpha;
+        x1 *= alpha;
+        if (F & EPI_BIAS) {
+          x0 += b0[j];
+          x1 += b1[j];
+        }
+        if (F & EPI_RELU) {
+          x0 = fmaxf(x0, 0.0f);
+          x1 = fmaxf(x1, 0.0f);
+        }
+        if (F & EPI_DROP_RNG) {
+          const uint64_t e = roff + (uint64_t)m * (uint64_t)N + (uint64_t)n;
+          bool k0, k1;
+          if ((e & 1ull) == 0) {        // the pair lies in one 4-column group of the RNG stream
+            const uint64_t hsh = rng_hash4(seed, step, e >> 2);
+            k0 = rng_keep_bits(hsh, (int)(e & 3ull), thr);
+            k1 = rng_keep_bits(hsh, (int)(e & 3ull) + 1, thr);
+          } else {
+            k0 = rng_keep(seed, step, e, dp);
+            k1 = rng_keep(seed, step, e + 1, dp);
+          }
+          const float f0 = k0 ? dscale : 0.0f, f1 = k1 ? dscale : 0.0f;
+          x0 = f0 != 0.0f ? x0 * f0 : 0.0f;
+          x1 = f1 != 0.0f ? x1 * f1 : 0.0f;
+        }
+      } else {
+        x0 = epilogue_t<F>(g, m, n, x0);
+        if (two) x1 = epilogue_t<F>(g, m, n + 1, x1);
+      }
+      frag_st2(C + (size_t)m * ldc + n, x0, x1, vec, two);
+    }
+  }
+}
+
+// The finished tile (all 256 consumer threads; tile origin tm0, tn0).  Unsplit: epilogue -> C.  Split: raw partial
+// -> partial[split] (the separate fixed-order reduce pass applies the epilogue).
+__device__ __forceinline__ void frag_finish(const Group& g, const int split, const int tm0, const int tn0,
+                                            const float (&v)[64]) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m0 = tm0 + (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2), n0 = tn0 + 2 * (lane & 3);
+  if (g.ksplit > 1) {
+    const int M = g.M, N = g.N;
+    float* const part = g.partial + (size_t)split * M * N;
+    const bool vec = (N % 2) == 0;          // partial planes are 256-B aligned
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int m = m0 + 8 * h, n = n0 + 8 * j;
+        if (m < M && n < N) frag_st2(part + (size_t)m * N + n, v[4 * j + 2 * h], v[4 * j + 2 * h + 1], vec, n + 1 < N);
+      }
+    return;
+  }
+  TA3N_EPI_DISPATCH(g.flags, { frag_epilogue<EPI_F>(g, m0, n0, v); })
+}
+
+// ---- the plain kernel ("tf32"): one tile per CTA ---------------------------------------------------------------
+// Warp 8 lane 0 issues the TMA loads; for MN-major B, warps 9..11 write the K-major copy of each landed B tile beside
+// it and mark the stage ready.  The consumers load their A fragments from the landed A tile (either layout) and issue
+// one product per K step with B from shared memory: they do nothing else in the K loop.  Per slab and CTA, shared
+// memory moves 32 KB of TMA fill, 16 KB of A fragment loads and 32 KB of B operand reads (each warpgroup reads all of
+// B), + 32 KB for the transpose of MN-major B.
+
+// Consumer warpgroups: slab `it` of the tile, A fragments in `a` (not the set of the group still in flight).  Leaves
+// this slab's group in flight and releases the previous stage.
+template <bool A_KMAJ, bool B_KMAJ>
+__device__ __forceinline__ void tc_consume_slab(const uint32_t it, uint8_t* smem, TcShared* sh, uint64_t* ready_bar,
+                                                const uint32_t off0, const uint32_t off1, uint32_t (&a)[16],
+                                                float (&d)[64], int& prev) {
+  const int stage = (int)(it % TC_STAGES);
+  const uint32_t parity = (it / TC_STAGES) & 1u;
+  mbar_wait(&sh->full_bar[stage], parity);          // A landed (read below with ordinary loads)
+  if (!B_KMAJ) mbar_wait(&ready_bar[stage], parity);  // K-major copy of B written
+  const uint32_t a_base = smem_u32(smem + stage * tc_stage_bytes(B_KMAJ));
+  const uint32_t b_base = a_base + TC_A_BYTES + (B_KMAJ ? 0 : TC_B_BYTES);
+  tc_load_a<A_KMAJ>(a_base, off0, off1, a);
+#pragma unroll
+  for (int j = 0; j < 16; ++j) reg_fence(a[j]);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < TC_BK / 8; ++ks) {
+    const int f = 4 * ks;
+    wgmma_tf32_rs(d, a[f], a[f + 1], a[f + 2], a[f + 3], wgmma_desc(b_base, ks));
+  }
+  wgmma_commit();
+  wgmma_wait<1>();                                  // the previous slab's MMAs are done: release its stage
+  if (prev >= 0) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&sh->empty_bar[prev]);
+  }
+  prev = stage;
+}
+
 template <bool A_KMAJ, bool B_KMAJ>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 seg_gemm_tc_kernel(const __grid_constant__ GemmTable tab, const __grid_constant__ TcMaps maps,
                    const __grid_constant__ TcSegMaps segmaps, const int first_wave) {
+  constexpr int kStageBytes = tc_stage_bytes(B_KMAJ);
   extern __shared__ uint8_t tc_smem_raw[];
   __shared__ __align__(8) TcShared sh;
+  __shared__ __align__(8) uint64_t ready_bar[TC_STAGES];     // B transposed (one arrival per B warp)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -454,24 +511,56 @@ seg_gemm_tc_kernel(const __grid_constant__ GemmTable tab, const __grid_constant_
   tc_decode(ctx, tile, &split, &m0, &n0);
   tc_chunk_range(ctx, split, &c_begin, &n_iter);
 
-  if (warp == TC_CONSUMER_WARPS && lane == 0) tc_pipe_init<TC_STAGES>(&sh);
+  if (warp == TC_CONSUMER_WARPS && lane == 0) {
+    for (int s = 0; s < TC_STAGES; ++s) mbar_init(&ready_bar[s], TC_B_WARPS);
+    tc_pipe_init<TC_STAGES>(&sh);
+  }
   __syncthreads();
   // Everything above touched only kernel parameters and shared memory: it overlaps the previous kernel of the
   // stream.  From here on operands produced by that kernel are read.
   pdl_wait();
 
-  const int mode = ctx.g.ksplit > 1 ? TILE_PARTIAL : TILE_FINAL;
-  if (warp == TC_CONSUMER_WARPS) {
-    if (lane == 0 && n_iter > 0)
-      tc_produce<TC_STAGES>(ctx, maps.m, A_KMAJ, B_KMAJ, tab.pad_, m0, n0, c_begin, n_iter, smem, &sh, 0u);
+  if (warp >= TC_CONSUMER_WARPS) {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (warp == TC_CONSUMER_WARPS) {
+      if (lane == 0 && n_iter > 0)
+        tc_produce<TC_STAGES, kStageBytes>(ctx, maps.m, A_KMAJ, B_KMAJ, tab.pad_, m0, n0, c_begin, n_iter, smem, &sh,
+                                           0u);
+    } else if (!B_KMAJ) {
+      const int t = threadIdx.x - 32 * (TC_CONSUMER_WARPS + 1);
+      for (int it = 0; it < n_iter; ++it) {
+        const int stage = it % TC_STAGES;
+        mbar_wait(&sh.full_bar[stage], (uint32_t)(it / TC_STAGES) & 1u);
+        const uint32_t b_mn = smem_u32(smem + stage * kStageBytes) + TC_A_BYTES;
+        tc_transpose_b(b_mn, b_mn + TC_B_BYTES, t);
+        fence_proxy_async();            // generic-proxy writes -> the tensor core's reads
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&ready_bar[stage]);
+      }
+    }
   } else {
+    setmaxnreg_inc<TC_CONSUMER_REGS>();
+    const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);      // fragment rows r0, r0 + 8
+    const uint32_t off0 = tc_a_thread_off<A_KMAJ>(r0, lane & 3), off1 = tc_a_thread_off<A_KMAJ>(r0 + 8, lane & 3);
     float d[64];
-    tc_consume<TC_STAGES>(A_KMAJ, B_KMAJ, n_iter, smem, &sh, d);
-    consumer_sync();                    // every MMA has read the ring: it becomes the accumulator tile
-    float* acc = reinterpret_cast<float*>(smem);
-    tc_store_acc(acc, d, threadIdx.x);
-    consumer_sync();
-    tc_epilogue<TC_CONSUMER_WARPS>(ctx, m0, n0, split, n_iter, mode, acc, warp);
+#pragma unroll
+    for (int j = 0; j < 64; ++j) d[j] = 0.f;
+    uint32_t a[2][16];                  // A fragments of the even / odd slabs
+    int prev = -1;                      // stage whose MMAs may still be in flight
+    // The odd last slab is peeled off the loop: with the pair's second slab conditional inside it, the back edge would
+    // let one register set be rewritten while its own group is in flight, and ptxas would serialize every MMA (C7513).
+    int it = 0;
+    for (; it + 1 < n_iter; it += 2) {
+      tc_consume_slab<A_KMAJ, B_KMAJ>((uint32_t)it, smem, &sh, ready_bar, off0, off1, a[0], d, prev);
+      tc_consume_slab<A_KMAJ, B_KMAJ>((uint32_t)(it + 1), smem, &sh, ready_bar, off0, off1, a[1], d, prev);
+    }
+    if (it < n_iter) tc_consume_slab<A_KMAJ, B_KMAJ>((uint32_t)it, smem, &sh, ready_bar, off0, off1, a[0], d, prev);
+    wgmma_wait<0>();
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&sh.empty_bar[prev]);
+    }
+    frag_finish(ctx.g, split, m0, n0, d);
   }
 }
 
@@ -493,13 +582,6 @@ seg_gemm_tc_kernel(const __grid_constant__ GemmTable tab, const __grid_constant_
 // the three products with B from shared memory.  The consumer warps do nothing else in the K loop; they fold every
 // finished chunk into 64 running sums.  setmaxnreg moves registers from the producer warpgroup to the consumers,
 // which hold 64 accumulators, 64 sums and two slabs of A fragments (hi and lo).
-constexpr int X3_THREADS = 384;                               // warps 0..7 consumers, 8 TMA, 9..11 B split
-constexpr int X3_SPLIT_WARPS = 3;
-constexpr int X3_SPLIT_THREADS = 32 * X3_SPLIT_WARPS;
-// one CTA per SM: 65536 / 384 threads, rounded down to the allocation unit of 8, is 168 registers per thread at launch
-constexpr int X3_PRODUCER_REGS = 40, X3_CONSUMER_REGS = 232;
-static_assert(128 * X3_PRODUCER_REGS + 256 * X3_CONSUMER_REGS <= X3_THREADS * 168,
-              "setmaxnreg budget exceeds the registers of one CTA");
 constexpr int X3_STAGES = 4;
 constexpr int X3_STAGE_BYTES = TC_STAGE_BYTES + TC_B_BYTES;   // [A raw | B raw (= B hi) | B lo]
 constexpr int X3_CHUNK = 8;                                   // slabs (256 K columns) per tensor-core accumulation
@@ -576,51 +658,30 @@ template <bool B_KMAJ>
 __device__ __forceinline__ void x3_split_b(const uint32_t b_raw, const uint32_t b_lo, const int t) {
   uint32_t src = b_raw;
   if (!B_KMAJ) {
-#pragma unroll 1
-    for (int blk = t; blk < 256; blk += X3_SPLIT_THREADS) {
-      float4 r[4];
-      tc_prep_load(b_raw, blk, r);
-      tc_prep_store(b_lo, blk, r);
-    }
+    tc_transpose_b(b_raw, b_lo, t);
     x3_split_sync();                  // every read of the raw tile before the K-major writes over it
     src = b_lo;
   }
 #pragma unroll 2
-  for (int c = t; c < TC_B_BYTES / 16; c += X3_SPLIT_THREADS) {
+  for (int c = t; c < TC_B_BYTES / 16; c += TC_B_THREADS) {
     const float4 v = lds4(src + 16u * c);
     if (!B_KMAJ) sts4(b_raw + 16u * c, v);
     sts4(b_lo + 16u * c, make_float4(v.x - tf32_hi(v.x), v.y - tf32_hi(v.y), v.z - tf32_hi(v.z), v.w - tf32_hi(v.w)));
   }
 }
 
-// Per-thread part of the A fragment addresses of rows m = r0 (and r0 + 8, MN-major), column k = tq: the word offset
-// in the raw tile, whose bits 4..6 are the SW128 chunk index.  Stage bases are 1024-B aligned, so x3_load_a reaches
-// every other column by an XOR on those bits plus a constant, with no per-column offsets kept in registers.
-template <bool A_KMAJ>
-__device__ __forceinline__ uint32_t x3_a_thread_off(const int m, const int tq) {
-  return A_KMAJ ? kmaj_chunk(m, 0) + 4u * tq : mnmaj_chunk(tq, m >> 2) + 4u * (m & 3);
-}
-
-// Consumer thread: the A fragments of one slab (4 k-steps x 4 words, see wgmma_tf32_rs) from the raw stage, split
-// into hi and lo.  K-major loads are conflict-free (the SW128 chunk index differs per row), MN-major ones 2-way.
-//   K-major  (m, k = 8 ks + 4 half + tq): (a_raw + off0) ^ ((2 ks + half) << 4), + 1024 for row r0 + 8 (same m & 7)
-//   MN-major (m, k = 8 ks + 4 half + tq): (a_raw + off_m) ^ (half << 6), + 128 (4 half + 8 ks) k-rows
+// Consumer thread: the A fragments of one slab from the raw stage, split into hi and lo.
 template <bool A_KMAJ>
 __device__ __forceinline__ void x3_load_a(const uint32_t a_raw, const uint32_t off0, const uint32_t off1,
                                           uint32_t (&hi)[16], uint32_t (&lo)[16]) {
-  const uint32_t p0 = a_raw + off0, p1 = a_raw + off1;
+  uint32_t raw[16];
+  tc_load_a<A_KMAJ>(a_raw, off0, off1, raw);
 #pragma unroll
-  for (int ks = 0; ks < TC_BK / 8; ++ks)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const uint32_t row = j & 1, half = j >> 1;
-      const uint32_t addr = A_KMAJ ? (p0 ^ ((2u * ks + half) << 4)) + 1024u * row
-                                   : ((row ? p1 : p0) ^ (half << 6)) + 512u * half + 1024u * ks;
-      const float a = lds1(addr);
-      const float h = tf32_hi(a);
-      hi[4 * ks + j] = __float_as_uint(h);
-      lo[4 * ks + j] = __float_as_uint(a - h);
-    }
+  for (int j = 0; j < 16; ++j) {
+    const float a = __uint_as_float(raw[j]), h = tf32_hi(a);
+    hi[j] = __float_as_uint(h);
+    lo[j] = __float_as_uint(a - h);
+  }
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     reg_fence(hi[j]);
@@ -659,109 +720,8 @@ __device__ __forceinline__ void x3_consume_slab(const uint32_t gl, uint8_t* smem
   prev = stage;
 }
 
-// ---- epilogue straight from the accumulator fragment (consumer thread) ------------------------------------------
-// Thread (warp w, lane l) holds rows r0 = 64 (w / 4) + 16 (w % 4) + l / 4 and r0 + 8 of the tile, columns
-// 8j + 2(l % 4) + {0, 1} (see wgmma_tf32): v[4j + 2h + e] = (row r0 + 8h, column c0 + 8j + e), c0 = 2(l % 4).  A warp
-// store instruction then covers 8 rows x 32 B, whole sectors.
-__device__ __forceinline__ void x3_st2(float* p, const float x0, const float x1, const bool vec, const bool two) {
-  if (vec) {
-    *reinterpret_cast<float2*>(p) = make_float2(x0, x1);
-  } else {
-    p[0] = x0;
-    if (two) p[1] = x1;
-  }
-}
-
-// The fused epilogue of the fragment -> C.  The forward flag sets (bias, ReLU, RNG dropout) work from register copies
-// of the group fields and draw one rng_hash4 per 4-column group; every other set applies epilogue_t per element.
-template <int F>
-__device__ __forceinline__ void x3_epilogue(const Group& g, const int m0, const int n0, const float (&v)[64]) {
-  constexpr bool kFwd = F >= 0 && (F & ~(EPI_BIAS | EPI_RELU | EPI_DROP_RNG)) == 0;
-  const int M = g.M, N = g.N, ldc = g.ldc;
-  float* const C = g.C;
-  const bool vec = (N % 2) == 0 && (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) & 7u) == 0;
-  const float alpha = kFwd ? (g.alpha_dev ? g.alpha * __ldg(g.alpha_dev) : g.alpha) : 0.f;
-  const float* const bias = g.bias;
-  const uint64_t seed = g.seed, roff = g.rng_offset;
-  const uint64_t step = (kFwd && (F & EPI_DROP_RNG) && g.step_dev) ? *g.step_dev : 0ull;
-  const float dscale = g.drop_scale, dp = g.drop_p;
-  const uint32_t thr = rng_threshold(dp);
-  float b0[16], b1[16];                 // bias of the thread's columns, loaded before the first store
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const int n = n0 + 8 * j;
-    b0[j] = kFwd && (F & EPI_BIAS) && n < N ? bias[n] : 0.f;
-    b1[j] = kFwd && (F & EPI_BIAS) && n + 1 < N ? bias[n + 1] : 0.f;
-  }
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int m = m0 + 8 * h;
-    if (m >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int n = n0 + 8 * j;
-      if (n >= N) continue;
-      const bool two = n + 1 < N;
-      float x0 = v[4 * j + 2 * h], x1 = v[4 * j + 2 * h + 1];
-      if (kFwd) {
-        x0 *= alpha;
-        x1 *= alpha;
-        if (F & EPI_BIAS) {
-          x0 += b0[j];
-          x1 += b1[j];
-        }
-        if (F & EPI_RELU) {
-          x0 = fmaxf(x0, 0.0f);
-          x1 = fmaxf(x1, 0.0f);
-        }
-        if (F & EPI_DROP_RNG) {
-          const uint64_t e = roff + (uint64_t)m * (uint64_t)N + (uint64_t)n;
-          bool k0, k1;
-          if ((e & 1ull) == 0) {        // the pair lies in one 4-column group of the RNG stream
-            const uint64_t hsh = rng_hash4(seed, step, e >> 2);
-            k0 = rng_keep_bits(hsh, (int)(e & 3ull), thr);
-            k1 = rng_keep_bits(hsh, (int)(e & 3ull) + 1, thr);
-          } else {
-            k0 = rng_keep(seed, step, e, dp);
-            k1 = rng_keep(seed, step, e + 1, dp);
-          }
-          const float f0 = k0 ? dscale : 0.0f, f1 = k1 ? dscale : 0.0f;
-          x0 = f0 != 0.0f ? x0 * f0 : 0.0f;
-          x1 = f1 != 0.0f ? x1 * f1 : 0.0f;
-        }
-      } else {
-        x0 = epilogue_t<F>(g, m, n, x0);
-        if (two) x1 = epilogue_t<F>(g, m, n + 1, x1);
-      }
-      x3_st2(C + (size_t)m * ldc + n, x0, x1, vec, two);
-    }
-  }
-}
-
-// The finished task (all 256 consumer threads).  Unsplit: epilogue -> C.  Split: raw partial -> partial[split] (the
-// separate fixed-order reduce pass applies the epilogue).
-__device__ __forceinline__ void x3_finish(const X3Slot& sl, const float (&v)[64]) {
-  const Group& g = sl.ctx.g;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = sl.m0 + (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2), n0 = sl.n0 + 2 * (lane & 3);
-  if (g.ksplit > 1) {
-    const int M = g.M, N = g.N;
-    float* const part = g.partial + (size_t)sl.split * M * N;
-    const bool vec = (N % 2) == 0;          // partial planes are 256-B aligned
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int m = m0 + 8 * h, n = n0 + 8 * j;
-        if (m < M && n < N) x3_st2(part + (size_t)m * N + n, v[4 * j + 2 * h], v[4 * j + 2 * h + 1], vec, n + 1 < N);
-      }
-    return;
-  }
-  TA3N_EPI_DISPATCH(g.flags, { x3_epilogue<EPI_F>(g, m0, n0, v); })
-}
-
 template <bool A_KMAJ, bool B_KMAJ>
-__global__ void __launch_bounds__(X3_THREADS, 1)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 seg_gemm_tc_x3_kernel(const __grid_constant__ GemmTable tab, const __grid_constant__ TcMaps maps,
                       const __grid_constant__ TcSegMaps segmaps, const __grid_constant__ X3Sched sched) {
   extern __shared__ uint8_t tc_smem_raw[];
@@ -777,7 +737,7 @@ seg_gemm_tc_x3_kernel(const __grid_constant__ GemmTable tab, const __grid_consta
 
   if (warp == TC_CONSUMER_WARPS) {
     if (lane == 0) {
-      for (int s = 0; s < X3_STAGES; ++s) mbar_init(&ready_bar[s], X3_SPLIT_WARPS);
+      for (int s = 0; s < X3_STAGES; ++s) mbar_init(&ready_bar[s], TC_B_WARPS);
       for (int s = 0; s < 2; ++s) {
         mbar_init(&slot_full[s], 1);
         mbar_init(&slot_empty[s], X3_SLOT_READERS);
@@ -794,7 +754,7 @@ seg_gemm_tc_x3_kernel(const __grid_constant__ GemmTable tab, const __grid_consta
   pdl_wait();
 
   if (warp >= TC_CONSUMER_WARPS) {
-    setmaxnreg_dec<X3_PRODUCER_REGS>();
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
     uint32_t slabs = 0;                 // slabs of the CTA so far: ring stage and parity
     if (warp == TC_CONSUMER_WARPS) {
       for (int k = 0; k < n_tasks; ++k) {
@@ -833,9 +793,9 @@ seg_gemm_tc_x3_kernel(const __grid_constant__ GemmTable tab, const __grid_consta
       }
     }
   } else {
-    setmaxnreg_inc<X3_CONSUMER_REGS>();
+    setmaxnreg_inc<TC_CONSUMER_REGS>();
     const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);      // fragment rows r0, r0 + 8
-    const uint32_t off0 = x3_a_thread_off<A_KMAJ>(r0, lane & 3), off1 = x3_a_thread_off<A_KMAJ>(r0 + 8, lane & 3);
+    const uint32_t off0 = tc_a_thread_off<A_KMAJ>(r0, lane & 3), off1 = tc_a_thread_off<A_KMAJ>(r0 + 8, lane & 3);
     uint32_t slabs = 0;
     for (int k = 0; k < n_tasks; ++k) {
       const int s = k & 1;
@@ -866,7 +826,7 @@ seg_gemm_tc_x3_kernel(const __grid_constant__ GemmTable tab, const __grid_consta
         }
       }
       slabs += (uint32_t)n_iter;
-      x3_finish(slots[s], sum);
+      frag_finish(slots[s].ctx.g, slots[s].split, slots[s].m0, slots[s].n0, sum);
       __syncwarp();
       if (lane == 0) mbar_arrive(&slot_empty[s]);
     }
@@ -1016,13 +976,13 @@ inline int tc_launch_one(const GemmTable& tab, const TcMaps& maps, const TcSegMa
     if (!d) return fail(TA3N_ERR_CUDA, "cudaGetDevice failed");
     if (!d->configured[slot]) {
       TA3N_CUDA(cudaFuncSetAttribute(seg_gemm_tc_kernel<A_KMAJ, B_KMAJ>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     tc_smem_bytes(TC_STAGES)));
+                                     tc_smem_bytes(B_KMAJ)));
       d->configured[slot] = true;
     }
     first_wave = d->sm_count;
   }
   pre_launch(label, stream);
-  launch_kernel(seg_gemm_tc_kernel<A_KMAJ, B_KMAJ>, tab.total_tiles, TC_THREADS, tc_smem_bytes(TC_STAGES), stream, tab,
+  launch_kernel(seg_gemm_tc_kernel<A_KMAJ, B_KMAJ>, tab.total_tiles, TC_THREADS, tc_smem_bytes(B_KMAJ), stream, tab,
                 maps, sm, first_wave);
   return after_launch();
 }
@@ -1043,7 +1003,7 @@ inline int tc_launch_x3(const GemmTable& tab, const TcMaps& maps, const TcSegMap
     }
   }
   pre_launch(label, stream);
-  launch_kernel(seg_gemm_tc_x3_kernel<A_KMAJ, B_KMAJ>, grid, X3_THREADS, x3_smem_bytes(), stream, tab, maps, sm, sched);
+  launch_kernel(seg_gemm_tc_x3_kernel<A_KMAJ, B_KMAJ>, grid, TC_THREADS, x3_smem_bytes(), stream, tab, maps, sm, sched);
   return after_launch();
 }
 

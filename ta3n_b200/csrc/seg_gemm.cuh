@@ -145,180 +145,6 @@ __device__ __forceinline__ float apply_epilogue(const Group& g, int m, int n, fl
   return epilogue_t<-1>(g, m, n, acc);
 }
 
-// 32 consecutive floats p[0..31] of one row -> registers; 16 B vector loads when possible.  ld.global.cg: read at L2
-// (no reuse in L1 anyway).
-__device__ __forceinline__ void load_row32(const float* p, int nvalid, float (&r)[32]) {
-  if (nvalid >= 32 && (reinterpret_cast<uintptr_t>(p) & 15u) == 0) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      const float4 t = __ldcg(reinterpret_cast<const float4*>(p + j));
-      r[j] = t.x;
-      r[j + 1] = t.y;
-      r[j + 2] = t.z;
-      r[j + 3] = t.w;
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) r[j] = j < nvalid ? __ldcg(p + j) : 0.f;
-  }
-}
-
-// dropout factor of the 32 elements (m, nb .. nb+31): mask bytes or the counter-based RNG
-__device__ __forceinline__ void drop_row32(const Group& g, const int f, int m, int nb, int nvalid, float (&v)[32]) {
-  if (f & EPI_DROP_MASK) {
-    const uint8_t* k = g.keep + (size_t)m * g.ldkeep + nb;
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (j < nvalid) v[j] = k[j] ? v[j] * g.drop_scale : 0.0f;
-  }
-  if (f & EPI_DROP_RNG) {
-    const uint64_t step = g.step_dev ? *g.step_dev : 0ull;
-    const uint64_t base = g.rng_offset + (uint64_t)m * (uint64_t)g.N + (uint64_t)nb;
-    if ((base & 3ull) == 0) {
-      const uint32_t thr = rng_threshold(g.drop_p);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const uint64_t hsh = rng_hash4(g.seed, step, (base + j) >> 2);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) v[j + i] = rng_keep_bits(hsh, i, thr) ? v[j + i] * g.drop_scale : 0.0f;
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = rng_keep(g.seed, step, base + j, g.drop_p) ? v[j] * g.drop_scale : 0.0f;
-    }
-  }
-}
-
-// The same epilogue applied to a 32-column segment (m, nb..nb+31) held by one thread (tensor-core engine: one
-// accumulator row per lane).  Auxiliary operands (bias, add, gate, C) are fetched as whole 128 B row pieces
-// with vector loads up front instead of one dependent scalar load per element.
-// generic form (flags read at run time; rare flag sets only): one auxiliary row at a time, few registers
-__device__ __forceinline__ void epilogue_row32_generic(const Group& g, int m, int nb, int nvalid, float (&v)[32]) {
-  const int f = g.flags;
-  float aux[32];
-  const float alpha = g.alpha_dev ? g.alpha * __ldg(g.alpha_dev) : g.alpha;
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] *= alpha;
-  if (f & EPI_BIAS) {
-    load_row32(g.bias + nb, nvalid, aux);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] += aux[j];
-  }
-  if (f & EPI_RELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.0f);
-  }
-  if ((f & (EPI_DROP_MASK | EPI_DROP_RNG)) && !(f & EPI_DROP_LATE)) drop_row32(g, f, m, nb, nvalid, v);
-  if (f & EPI_ADDROW) {
-    const float rs = g.rowscale ? __ldcg(g.rowscale + (size_t)m * g.rs_stride) + g.rs_bias : 1.0f;
-    load_row32(g.add + (size_t)m * g.ldadd + nb, nvalid, aux);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaf(rs, aux[j], v[j]);
-  }
-  if ((f & (EPI_DROP_MASK | EPI_DROP_RNG)) && (f & EPI_DROP_LATE)) drop_row32(g, f, m, nb, nvalid, v);
-  if (f & EPI_GATE) {
-    load_row32(g.gate + (size_t)m * g.ldgate + nb, nvalid, aux);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = aux[j] > 0.0f ? v[j] : 0.0f;
-  }
-  if (f & EPI_ACCUM) {
-    load_row32(g.C + (size_t)m * g.ldc + nb, nvalid, aux);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] += aux[j];
-  }
-  if (f & EPI_DPRE) {
-    load_row32(g.gate + (size_t)m * g.ldgate + nb, nvalid, aux);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = aux[j] > 0.0f ? v[j] * g.drop_scale : 0.0f;
-  }
-  if (f & EPI_MULTI) {
-#pragma unroll
-    for (int q = 0; q < 3; ++q) {
-      if (q >= g.n_multi) break;
-      load_row32(g.multi_gate[q] + (size_t)m * g.ldmulti + nb, nvalid, aux);
-      float* o = g.multi_out[q] + (size_t)m * g.ldmulti + nb;
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (j < nvalid) o[j] = aux[j] > 0.f ? v[j] : 0.f;
-    }
-  }
-}
-
-template <int F>
-__device__ __forceinline__ void epilogue_row32(const Group& g, int m, int nb, int nvalid, float (&v)[32]) {
-  if (F < 0) {
-    epilogue_row32_generic(g, m, nb, nvalid, v);
-    return;
-  }
-  const int f = F;
-  // Every auxiliary row this flag set needs is requested BEFORE the first one is used: the epilogue is a chain of
-  // L2 round trips (~0.4 us each) otherwise -- five of them for the relation-discriminator data gradient.
-  float a_bias[32], a_add[32], a_gate[32], a_c[32];
-  float rs = 1.0f;
-  if (f & EPI_BIAS) load_row32(g.bias + nb, nvalid, a_bias);
-  if (f & EPI_ADDROW) {
-    if (g.rowscale) rs = __ldcg(g.rowscale + (size_t)m * g.rs_stride) + g.rs_bias;
-    load_row32(g.add + (size_t)m * g.ldadd + nb, nvalid, a_add);
-  }
-  if (f & (EPI_GATE | EPI_DPRE)) load_row32(g.gate + (size_t)m * g.ldgate + nb, nvalid, a_gate);
-  if (f & EPI_ACCUM) load_row32(g.C + (size_t)m * g.ldc + nb, nvalid, a_c);
-  const float alpha = g.alpha_dev ? g.alpha * __ldg(g.alpha_dev) : g.alpha;
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] *= alpha;
-  if (f & EPI_BIAS) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] += a_bias[j];
-  }
-  if (f & EPI_RELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.0f);
-  }
-  if ((f & (EPI_DROP_MASK | EPI_DROP_RNG)) && !(f & EPI_DROP_LATE)) drop_row32(g, f, m, nb, nvalid, v);
-  if (f & EPI_ADDROW) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaf(rs, a_add[j], v[j]);
-  }
-  if ((f & (EPI_DROP_MASK | EPI_DROP_RNG)) && (f & EPI_DROP_LATE)) drop_row32(g, f, m, nb, nvalid, v);
-  if (f & EPI_GATE) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = a_gate[j] > 0.0f ? v[j] : 0.0f;
-  }
-  if (f & EPI_ACCUM) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] += a_c[j];
-  }
-  if (f & EPI_DPRE) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = a_gate[j] > 0.0f ? v[j] * g.drop_scale : 0.0f;
-  }
-  if (f & EPI_MULTI) {
-    // the gates of two planes in flight together (a_bias / a_add / a_c are dead by now: their registers are reused)
-#pragma unroll
-    for (int q0 = 0; q0 < 3; q0 += 2) {      // constant indices: the Group copy stays in registers
-      if (q0 >= g.n_multi) break;
-      float gq[2][32];
-#pragma unroll
-      for (int u = 0; u < 2; ++u)
-        if (q0 + u < 3 && q0 + u < g.n_multi) load_row32(g.multi_gate[q0 + u < 3 ? q0 + u : 2] + (size_t)m * g.ldmulti + nb, nvalid, gq[u]);
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        if (q0 + u >= 3 || q0 + u >= g.n_multi) break;
-        float* o = g.multi_out[q0 + u < 3 ? q0 + u : 2] + (size_t)m * g.ldmulti + nb;
-        if (nvalid >= 32 && (reinterpret_cast<uintptr_t>(o) & 15u) == 0) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(o + j) = make_float4(gq[u][j] > 0.f ? v[j] : 0.f, gq[u][j + 1] > 0.f ? v[j + 1] : 0.f,
-                                                            gq[u][j + 2] > 0.f ? v[j + 2] : 0.f, gq[u][j + 3] > 0.f ? v[j + 3] : 0.f);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (j < nvalid) o[j] = gq[u][j] > 0.f ? v[j] : 0.f;
-        }
-      }
-    }
-  }
-}
-
 // Call `body(tag)` with tag = std::integral_constant<int, F> for the flag set of `flags`.
 #define TA3N_EPI_DISPATCH(flags, ...)                                              \
   switch (flags) {                                                                  \
