@@ -106,6 +106,10 @@ size_t ta3n_timing_report(char* buf, size_t buf_bytes);
 int ta3n_shared_fc_fwd(const float* x_src, int rows_src, const float* x_tgt, int rows_tgt, int D,
                        const float* W, const float* b, int F, const ta3n_dropout* drop,
                        float* feat, ta3n_stream_t stream);
+/* A stacked shared layer (add_fc 2 and 3, models.py:581-603): ta3n_shared_fc_fwd with D = F, timed under its own
+ * call-site label.  x_src / x_tgt are the source / target rows of the layer below's output.                        */
+int ta3n_shared_fc_stack_fwd(const float* x_src, int rows_src, const float* x_tgt, int rows_tgt, const float* W,
+                             const float* b, int F, const ta3n_dropout* drop, float* feat, ta3n_stream_t stream);
 size_t ta3n_shared_fc_bwd_workspace_bytes(int rows, int D, int F);
 /* dfeat [rows, F] is consumed (overwritten with d pre-activation). Inputs carry no grad
  * (SURVEY 3.3) so only dW [F, D], db [F] are produced.                                   */
@@ -113,6 +117,14 @@ int ta3n_shared_fc_bwd(const float* x_src, int rows_src, const float* x_tgt, int
                        int F, const float* feat, float* dfeat, const float* g_feat_ext, float p,
                        float* dW, float* db, void* workspace, size_t workspace_bytes,
                        ta3n_stream_t stream);
+/* The same backward for a stacked shared layer (add_fc 2 and 3, models.py:581-603), whose input x = source | target
+ * rows of the layer below carries a gradient: dfeat is consumed as above, then dx [rows_src+rows_tgt, D] = dpre W is
+ * STORED (W [F, D]; not accumulated) before dW, db are formed, so that between ta3n_wgrad_defer_begin / _flush only
+ * dW and db are deferred.  rows == 0 zeroes dW, db.  Workspace: ta3n_shared_fc_bwd_workspace_bytes.               */
+int ta3n_shared_fc_bwd_dx(const float* x_src, int rows_src, const float* x_tgt, int rows_tgt, int D,
+                          int F, const float* W, const float* feat, float* dfeat, const float* g_feat_ext,
+                          float p, float* dx, float* dW, float* db, void* workspace, size_t workspace_bytes,
+                          ta3n_stream_t stream);
 
 /* ---- GradReverse + two-layer domain discriminator ---------------------------------- */
 /* models.py:456-462 (frame level), :464-470 (video level):

@@ -69,8 +69,10 @@ SIGNATURES = {
     "ta3n_timing_enable": (None, [_I]),
     "ta3n_timing_report": (_SZ, [C.c_char_p, _SZ]),
     "ta3n_shared_fc_fwd": (_I, [_VP, _I, _VP, _I, _I, _VP, _VP, _I, _DRP, _VP, _VP]),
+    "ta3n_shared_fc_stack_fwd": (_I, [_VP, _I, _VP, _I, _VP, _VP, _I, _DRP, _VP, _VP]),
     "ta3n_shared_fc_bwd_workspace_bytes": (_SZ, [_I, _I, _I]),
     "ta3n_shared_fc_bwd": (_I, [_VP, _I, _VP, _I, _I, _I, _VP, _VP, _VP, _F, _VP, _VP, _VP, _SZ, _VP]),
+    "ta3n_shared_fc_bwd_dx": (_I, [_VP, _I, _VP, _I, _I, _I, _VP, _VP, _VP, _VP, _F, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "ta3n_disc_fwd": (_I, [_VP, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "ta3n_disc_bwd_workspace_bytes": (_SZ, [_I, _I, _I]),
     "ta3n_disc_bwd": (_I, [_VP, _I, _I, _I, _VP, _VP, _VP, _VP, _F, _VP, _I, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),

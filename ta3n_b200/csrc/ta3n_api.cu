@@ -286,15 +286,17 @@ size_t ta3n_timing_report(char* buf, size_t buf_bytes) {
 // ------------------------------------------------------------------------------------------------
 // shared frame layer                                                        models.py:565-575
 // ------------------------------------------------------------------------------------------------
-int ta3n_shared_fc_fwd(const float* x_src, int rows_src, const float* x_tgt, int rows_tgt, int D,
-                       const float* W, const float* b, int F, const ta3n_dropout* drop, float* feat,
-                       ta3n_stream_t stream) {
+}  // extern "C"
+
+namespace {
+int shared_fc_fwd(const float* x_src, int rows_src, const float* x_tgt, int rows_tgt, int D, const float* W,
+                  const float* b, int F, const ta3n_dropout* drop, float* feat, cudaStream_t stream, const char* label) {
   TA3N_REQUIRE(rows_src >= 0 && rows_tgt >= 0 && D > 0 && F > 0, "bad sizes");
   TA3N_REQUIRE(W && b && feat, "null pointer");
   TA3N_REQUIRE((rows_src == 0 || x_src) && (rows_tgt == 0 || x_tgt), "null input");
   const DropArgs d = make_drop(drop);
   GemmPlan plan;
-    plan.label = "shared_fc_fwd";
+    plan.label = label;
     plan.precise = true;
   const float* xs[2] = {x_src, x_tgt};
   const int rows[2] = {rows_src, rows_tgt};
@@ -309,7 +311,22 @@ int ta3n_shared_fc_fwd(const float* x_src, int rows_src, const float* x_tgt, int
     }
     row0 += rows[dom];
   }
-  return run_gemm(plan, S(stream));
+  return run_gemm(plan, stream);
+}
+}  // namespace
+
+extern "C" {
+
+int ta3n_shared_fc_fwd(const float* x_src, int rows_src, const float* x_tgt, int rows_tgt, int D,
+                       const float* W, const float* b, int F, const ta3n_dropout* drop, float* feat,
+                       ta3n_stream_t stream) {
+  return shared_fc_fwd(x_src, rows_src, x_tgt, rows_tgt, D, W, b, F, drop, feat, S(stream), "shared_fc_fwd");
+}
+
+// a stacked shared layer (add_fc 2 and 3): the same layer with D = F, under its own call-site label
+int ta3n_shared_fc_stack_fwd(const float* x_src, int rows_src, const float* x_tgt, int rows_tgt, const float* W,
+                             const float* b, int F, const ta3n_dropout* drop, float* feat, ta3n_stream_t stream) {
+  return shared_fc_fwd(x_src, rows_src, x_tgt, rows_tgt, F, W, b, F, drop, feat, S(stream), "shared_fc_stack_fwd");
 }
 
 size_t ta3n_shared_fc_bwd_workspace_bytes(int rows, int D, int F) {
@@ -337,6 +354,55 @@ int ta3n_shared_fc_bwd(const float* x_src, int rows_src, const float* x_tgt, int
   Arena arena(workspace, workspace_bytes);
   GemmPlan plan;
     plan.label = "shared_fc_wgrad";
+  plan.a_kmaj = false;
+  plan.b_kmaj = false;
+  plan.add_group(F, D, dW, D);
+  if (rows_src > 0) plan.add_seg(dfeat, F, x_src, D, rows_src);
+  if (rows_tgt > 0) plan.add_seg(dfeat + (size_t)rows_src * F, F, x_tgt, D, rows_tgt);
+  TA3N_TRY(submit_wgrad(plan, S(stream), &arena));
+
+  ColsumPlan cs;
+  cs.add(db, F, F);
+  cs.seg(dfeat, rows);
+  return submit_colsum(cs, S(stream), &arena);
+}
+
+// The same backward for a layer whose input carries a gradient (the stacked layers 2 and 3 of add_fc > 1, models.py:
+// 581-603): after the d pre-activation pass, dx [rows, D] = dpre W goes on the chain, before the weight gradient, so
+// that ta3n_wgrad_defer_* defers only dW and db.  dx is stored (not accumulated); the layer below applies its own
+// ReLU / dropout gate and any external gradient on its output in its own d pre-activation pass.
+int ta3n_shared_fc_bwd_dx(const float* x_src, int rows_src, const float* x_tgt, int rows_tgt, int D, int F,
+                          const float* W, const float* feat, float* dfeat, const float* g_feat_ext, float p, float* dx,
+                          float* dW, float* db, void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
+  TA3N_REQUIRE(rows_src >= 0 && rows_tgt >= 0 && D > 0 && F > 0, "bad sizes");
+  TA3N_REQUIRE(dW && db, "null gradient pointer");
+  TA3N_REQUIRE(p >= 0.f && p < 1.f, "dropout p must be in [0,1)");
+  const int rows = rows_src + rows_tgt;
+  TA3N_REQUIRE(rows == 0 || (W && feat && dfeat && dx), "null pointer");
+  if (rows == 0) {
+    TA3N_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * F * D, S(stream)));
+    TA3N_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * F, S(stream)));
+    return TA3N_OK;
+  }
+  const size_t total = (size_t)rows * F;
+  pre_launch("shared_fc_stack_dpre", S(stream));
+  launch_dpre(feat, dfeat, g_feat_ext, 1.0f / (1.0f - p), total, S(stream));
+  TA3N_TRY(after_launch());
+
+  {  // dx [rows, D] = dpre [rows, F] W [F, D]
+    GemmPlan plan;
+    plan.label = "shared_fc_stack_dgrad";
+    plan.precise_dgrad = true;
+    plan.a_kmaj = true;
+    plan.b_kmaj = false;
+    plan.add_group(rows, D, dx, D);
+    plan.add_seg(dfeat, F, W, D, F);
+    TA3N_TRY(run_gemm(plan, S(stream)));
+  }
+
+  Arena arena(workspace, workspace_bytes);
+  GemmPlan plan;
+  plan.label = "shared_fc_stack_wgrad";
   plan.a_kmaj = false;
   plan.b_kmaj = false;
   plan.add_group(F, D, dW, D);

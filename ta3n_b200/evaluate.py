@@ -113,7 +113,7 @@ class EvalStep:
         self.spec = TF.PathSpec(num_segments=self.T, beta=(0.0, 0.0, 0.0), classify_only=True,
                                 use_attn=(model.use_attn == "TransAttn") if self.avgpool else model.use_attn != "none",
                                 general_attn=model.use_attn == "general",
-                                use_attn_frame=model.use_attn_frame != "none")
+                                use_attn_frame=model.use_attn_frame != "none", add_fc=int(getattr(model, "add_fc", 1)))
         if self.avgpool:
             self.R = 1                                  # the reference's attn output here: feat_video[:, 0] (:624-626)
         else:

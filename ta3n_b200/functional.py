@@ -186,6 +186,11 @@ class PathSpec:
     use_attn_frame: bool = False
     drop_i: DropSpec = field(default_factory=DropSpec)
     drop_v: DropSpec = field(default_factory=DropSpec)
+    # add_fc: the number of shared frame layers (models.py:141-153, 565-603).  Layers 2 and 3 take their W, b from
+    # behind the tensors the operator reads at add_fc=1; drop_stack holds their dropout_i (the same p as drop_i, an
+    # independent draw per layer; a layer without an entry runs without dropout)
+    add_fc: int = 1
+    drop_stack: Tuple[DropSpec, ...] = ()
     # the classification pass of ens_DA='MCD' (main.py:548-556): only the class logits feed its loss, so the video
     # discriminator is not run, nor the frame discriminator unless the frame attention reads it; with reverse and
     # mu == 0 nothing flows below the classifier (GRL_mu), so the backward stops at its weight gradient
@@ -196,12 +201,106 @@ class PathSpec:
 #   shared W,b | frame-disc W1,b1,W2,b2 | TRN W_0..W_{R-1} | TRN b_0..b_{R-1} |
 #   rel-disc W1_i | b1_i | W2_i | b2_i (each R long) | classifier W,b | video-disc W1,b1,W2,b2
 #   [ | attn_layer W1,b1,w2,b2  -- only with PathSpec.general_attn ]
-def _attn_layer_params(params, R):
-    """The four trailing tensors of the 'general' attention layer (models.py:320-325)."""
+#   [ | shared_2 W,b [ | shared_3 W,b ]  -- the stacked shared layers of add_fc 2 and 3 ]
+def _attn_layer_params(params, R, add_fc=1):
+    """The four tensors of the 'general' attention layer (models.py:320-325), behind the core ones."""
     n = 6 + 6 * R + 6
-    if len(params) != n + 4:
-        raise _lib.Ta3nError(f"general attention expects {n + 4} parameter tensors, got {len(params)}")
+    if len(params) != n + 4 + 2 * (add_fc - 1):
+        raise _lib.Ta3nError(f"general attention at add_fc={add_fc} expects {n + 4 + 2 * (add_fc - 1)} parameter "
+                             f"tensors, got {len(params)}")
     return params[n:n + 4]
+
+
+def _stack_params(params, n_core, add_fc):
+    """[(W_2, b_2), (W_3, b_3)][:add_fc - 1]: the stacked shared layers' tensors, appended behind the ``n_core`` tensors
+    the operator takes at add_fc=1."""
+    if not 1 <= add_fc <= 3:
+        raise _lib.Ta3nError(f"add_fc must be 1, 2 or 3 (models.py:141-153), got {add_fc}")
+    n = n_core + 2 * (add_fc - 1)
+    if len(params) != n:
+        raise _lib.Ta3nError(f"add_fc={add_fc} expects {n} parameter tensors, got {len(params)}")
+    return [(params[i], params[i + 1]) for i in range(n_core, n, 2)]
+
+
+def _n_core(spec: "PathSpec", R: int) -> int:
+    return 6 + 6 * R + 6 + (4 if spec.general_attn else 0)
+
+
+def _layer_drop(spec: "PathSpec", layer: int) -> "DropSpec":
+    if layer == 1:
+        return spec.drop_i
+    return spec.drop_stack[layer - 2] if len(spec.drop_stack) > layer - 2 else DropSpec()
+
+
+def shared_stack_forward(spec: "PathSpec", xs, xt, w_sh, b_sh, stack, bufs: "Buffers"):
+    """The shared frame layers 1..L (models.py:565-603), each Dropout(ReLU(x W^T + b)) with its own dropout draw; layers
+    2..L read the layer below's output, whose rows are source | target as well.  Returns their outputs, bottom first;
+    the last one is what the frame level reads.  Buffers: 'feat' for the top layer, 'feat_<l>' for layer l below it."""
+    lib = _lib.load()
+    st = _stream()
+    T = spec.num_segments
+    Bs, Bt, D = xs.shape[0], xt.shape[0], xs.shape[2]
+    M, F, L = Bs + Bt, w_sh.shape[0], 1 + len(stack)
+    feats = []
+    for layer in range(1, L + 1):
+        out = bufs.get("feat" if layer == L else f"feat_{layer}", M * T, F)
+        d = _layer_drop(spec, layer).cstruct()
+        if layer == 1:
+            check(lib.ta3n_shared_fc_fwd(_p(xs), Bs * T, _p(xt), Bt * T, D, _p(w_sh), _p(b_sh), F, _dref(d), _p(out), st))
+        else:
+            w, b = stack[layer - 2]
+            if tuple(w.shape) != (F, F) or tuple(b.shape) != (F,):
+                raise _lib.Ta3nError(f"shared layer {layer}: expected ({F}, {F}) and ({F},), got "
+                                     f"{tuple(w.shape)} and {tuple(b.shape)}")
+            x = feats[-1]
+            check(lib.ta3n_shared_fc_stack_fwd(_p(x), Bs * T, _p(x[Bs * T:]), Bt * T, _p(w), _p(b), F, _dref(d),
+                                               _p(out), st))
+        feats.append(out)
+    return feats
+
+
+def _stack_saved(feats):
+    """saved-tensor entries of the layers below the top one ('feat' itself is saved by the caller)."""
+    return {f"feat_{layer}": t for layer, t in enumerate(feats[:-1], start=1)}
+
+
+def _stack_outputs(feats, M, T, F):
+    """Outputs behind the operator's add_fc=1 outputs: feat_fc of layers L-1..1 (the reference's list order, :722)."""
+    return tuple(t.view(M, T, F) for t in reversed(feats[:-1]))
+
+
+def _stack_out_names(n_lower):
+    return tuple(f"feat_{layer}" for layer in range(n_lower, 0, -1))
+
+
+def shared_stack_backward(spec: "PathSpec", xs, xt, w_sh, stack, saved, d_feat, gin, dw_sh, db_sh, dstack,
+                          bufs: "Buffers"):
+    """Backward of shared_stack_forward, layer L..1.  ``d_feat``: the frame level's gradient on the top layer's output
+    (consumed); ``gin['feat']`` / ``gin['feat_<l>']``: external gradients on the top / layer l's output.  Layers L..2
+    write the data gradient of the layer below (ta3n_shared_fc_bwd_dx), which applies its own gate and external gradient
+    in its d pre-activation pass; layer 1's input carries no gradient (ta3n_shared_fc_bwd)."""
+    lib = _lib.load()
+    st = _stream()
+    T = spec.num_segments
+    Bs, Bt, D = xs.shape[0], xt.shape[0], xs.shape[2]
+    M, F, L = Bs + Bt, w_sh.shape[0], 1 + len(stack)
+    for layer in range(L, 0, -1):
+        feat = saved["feat"] if layer == L else saved[f"feat_{layer}"]
+        g_ext = gin.get("feat" if layer == L else f"feat_{layer}")
+        g_ext = None if g_ext is None else g_ext.reshape(M * T, F)
+        p = float(_layer_drop(spec, layer).p)
+        if layer == 1:
+            ws = bufs.workspace("shared", lib.ta3n_shared_fc_bwd_workspace_bytes(M * T, D, F))
+            check(lib.ta3n_shared_fc_bwd(_p(xs), Bs * T, _p(xt), Bt * T, D, F, _p(feat), _p(d_feat), _p(g_ext), p,
+                                         _p(dw_sh), _p(db_sh), _p(ws), ws.numel(), st))
+        else:
+            (w, _), (dw, db) = stack[layer - 2], dstack[layer - 2]
+            x = saved[f"feat_{layer - 1}"]
+            dx = bufs.get(f"d_feat_{layer - 1}", M * T, F)
+            ws = bufs.workspace(f"shared_{layer}", lib.ta3n_shared_fc_bwd_workspace_bytes(M * T, F, F))
+            check(lib.ta3n_shared_fc_bwd_dx(_p(x), Bs * T, _p(x[Bs * T:]), Bt * T, F, F, _p(w), _p(feat), _p(d_feat),
+                                            _p(g_ext), p, _p(dx), _p(dw), _p(db), _p(ws), ws.numel(), st))
+            d_feat = dx
 
 
 def _split_params(params, R):
@@ -257,13 +356,13 @@ def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: boo
     (w_sh, b_sh), (w1f, b1f, w2f, b2f), trn_w, trn_b, r_w1, r_b1, r_w2, r_b2, (w_c, b_c), \
         (w1v, b1v, w2v, b2v) = _split_params(params, R)
     F, H, Cn = w_sh.shape[0], trn_w[0].shape[0], w_c.shape[0]
+    stack = _stack_params(params, _n_core(spec, R), spec.add_fc)
     new = bufs.get
-    d_i, d_v = spec.drop_i.cstruct(), spec.drop_v.cstruct()
+    d_v = spec.drop_v.cstruct()
 
-    # 1. shared layer  (models.py:565-575)
-    feat = new("feat", M * T, F)
-    check(lib.ta3n_shared_fc_fwd(_p(xs), Bs * T, _p(xt), Bt * T, D, _p(w_sh), _p(b_sh), F, _dref(d_i),
-                                 _p(feat), st))
+    # 1. shared layers  (models.py:565-603); everything below reads the last one
+    feats = shared_stack_forward(spec, xs, xt, w_sh, b_sh, stack, bufs)
+    feat = feats[-1]
     # 2. frame-level discriminator  (models.py:606-610)
     frame_disc = not (spec.classify_only or stop_at_video_feature) or spec.use_attn_frame
     hid_f = pred_frame = None
@@ -298,7 +397,7 @@ def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: boo
     # 4b. 'general' attention (models.py:359-366, 379-388): the plain sum above + sum_r softmax_r(MLP(feat_rel)) feat_rel
     hid_a = None
     if spec.general_attn:
-        wa1, ba1, wa2, ba2 = _attn_layer_params(params, R)
+        wa1, ba1, wa2, ba2 = _attn_layer_params(params, R, spec.add_fc)
         hid_a = new("hid_a", M * R, H)
         check(lib.ta3n_general_attn_fwd(_p(feat_rel), M, R, H, _p(wa1), _p(ba1), _p(wa2), _p(ba2), _p(hid_a), _p(attn),
                                         _p(feat_video), st))
@@ -318,15 +417,17 @@ def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: boo
                  hid_r=hid_r, pred_rel=pred_rel, attn=attn, dropped=dropped, hid_v=hid_v)
     if hid_a is not None:
         saved["hid_a"] = hid_a
+    saved.update(_stack_saved(feats))
     outputs = (feat.view(M, T, F), None if pred_frame is None else pred_frame.view(M, T, 2), attn, pred_rel,
-               feat_video, pred_video, pred_dom_video, dropped)
+               feat_video, pred_video, pred_dom_video, dropped) + _stack_outputs(feats, M, T, F)
     return saved, outputs, (Bs, Bt, D, T, F, H, Cn)
 
 
 def path_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, bufs: Buffers, stage_done=None,
                   side_stream=None):
     """The backward C calls in their fixed order.  ``gin``: dict of incoming output gradients
-    (feat, pred_frame, attn, pred_rel, feat_video, pred_video, pred_dom_video; missing/None = zero).
+    (feat, pred_frame, attn, pred_rel, feat_video, pred_video, pred_dom_video, and feat_1 / feat_2 on the outputs of the
+    shared layers below the top one under add_fc > 1; missing/None = zero).
     ``gout``: list of tensors (same order as ``params``) that receive the parameter gradients.
     ``stage_done(name)`` (optional) is called after each module's calls ('video', 'relation', 'trn',
     'frame', 'shared') -- TrainStep uses it to issue the deferred weight-gradient work on a second stream.
@@ -407,8 +508,8 @@ def path_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, bufs: 
                                ptr_array([_p(t) for t in dr_b2]), _p(ws), ws.numel(), st))
     if spec.general_attn:
         # 4b'. the attention weights' own gradient: through softmax and the tanh MLP back into feat_rel
-        wa1, _, wa2, _ = _attn_layer_params(params, R)
-        dwa1, dba1, dwa2, dba2 = _attn_layer_params(gout, R)
+        wa1, _, wa2, _ = _attn_layer_params(params, R, spec.add_fc)
+        dwa1, dba1, dwa2, dba2 = _attn_layer_params(gout, R, spec.add_fc)
         ws = wsp("general_attn", lib.ta3n_general_attn_bwd_workspace_bytes(M, R, H))
         check(lib.ta3n_general_attn_bwd(_p(feat_rel), M, R, H, _p(wa1), _p(wa2), _p(saved["hid_a"]), _p(attn), _p(G),
                                         _p(g("attn")), _p(d_feat_rel), _p(dwa1), _p(dba1), _p(dwa2), _p(dba2),
@@ -436,16 +537,19 @@ def path_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, bufs: 
     if not frame_parallel and (not spec.classify_only or spec.use_attn_frame):
         frame_disc_bwd(st, 1)
     stage_done("frame")
-    # 1'. shared layer (wgrad only; the input features carry no gradient)
-    ws = wsp("shared", lib.ta3n_shared_fc_bwd_workspace_bytes(M * T, D, F))
-    g_feat = g("feat")
-    g_feat_flat = None if g_feat is None else g_feat.reshape(M * T, F)
-    check(lib.ta3n_shared_fc_bwd(_p(xs), Bs * T, _p(xt), Bt * T, D, F, _p(feat), _p(d_feat), _p(g_feat_flat),
-                                 float(spec.drop_i.p), _p(dw_sh), _p(db_sh), _p(ws), ws.numel(), st))
+    # 1'. shared layers L..1 (layer 1: wgrad only; the input features carry no gradient)
+    n_core = _n_core(spec, R)
+    shared_stack_backward(spec, xs, xt, w_sh, _stack_params(params, n_core, spec.add_fc), saved, d_feat, gin, dw_sh,
+                          db_sh, _stack_params(gout, n_core, spec.add_fc), bufs)
     stage_done("shared")
 
 
 _OUT_NAMES = ("feat", "pred_frame", "attn", "pred_rel", "feat_video", "pred_video", "pred_dom_video", "dropped")
+
+
+def _drop_keepalive(spec: PathSpec):
+    """The tensors the dropout descriptors point at, kept alive until the backward."""
+    return tuple(t for d in (spec.drop_i, spec.drop_v, *spec.drop_stack) for t in (d.keep, d.step))
 
 
 class _VideoPathFunction(torch.autograd.Function):
@@ -453,8 +557,9 @@ class _VideoPathFunction(torch.autograd.Function):
 
     Outputs (all for M = Bs + Bt rows, source rows first):
       feat_fc (M,T,F) | pred_frame (M,T,2) | attn (M,R) | pred_rel (M,R,2) | feat_video (M,H) |
-      pred_video (M,C) | pred_dom_video (M,2) | dropped (M,H): the video feature after dropout_v, for further heads
-    """
+      pred_video (M,C) | pred_dom_video (M,2) | dropped (M,H): the video feature after dropout_v, for further heads |
+      under add_fc > 1, feat_fc of the shared layers below the top one (M,T,F), layer L-1 first
+    (feat_fc is the top shared layer's output)"""
 
     @staticmethod
     def forward(ctx, spec: PathSpec, xs, xt, *params):
@@ -463,7 +568,8 @@ class _VideoPathFunction(torch.autograd.Function):
         saved, outputs, dims = path_forward(spec, xs, xt, params, Buffers(xs.device))
         ctx.spec, ctx.dims = spec, dims
         ctx.saved_names = list(saved)
-        ctx.drop_keepalive = (spec.drop_i.keep, spec.drop_v.keep, spec.drop_i.step, spec.drop_v.step)
+        ctx.out_names = _OUT_NAMES + _stack_out_names(len(outputs) - len(_OUT_NAMES))
+        ctx.drop_keepalive = _drop_keepalive(spec)
         ctx.save_for_backward(xs, xt, *[saved[k] for k in ctx.saved_names], *params)
         ctx.set_materialize_grads(False)
         return outputs
@@ -478,7 +584,7 @@ class _VideoPathFunction(torch.autograd.Function):
         n = len(ctx.saved_names)
         saved = dict(zip(ctx.saved_names, tensors[2:2 + n]))
         params = list(tensors[2 + n:])
-        gin = {k: _chk(g, "grad") for k, g in zip(_OUT_NAMES, grads) if g is not None}
+        gin = {k: _chk(g, "grad") for k, g in zip(ctx.out_names, grads) if g is not None}
         gout = [torch.empty_like(p) for p in params]
         path_backward(ctx.spec, ctx.dims, xs, xt, params, saved, gin, gout, Buffers(xs.device))
         return (None, None, None, *gout)
@@ -505,18 +611,19 @@ def avgpool_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, stop_at_video
     T = spec.num_segments
     if xs.dim() != 3 or xt.dim() != 3 or xs.shape[1] != T or xt.shape[1] != T or xs.shape[2] != xt.shape[2]:
         raise _lib.Ta3nError(f"inputs must be (B,{T},D); got {tuple(xs.shape)} and {tuple(xt.shape)}")
-    if len(params) != 12:
-        raise _lib.Ta3nError(f"the avgpool path takes 12 parameter tensors, got {len(params)}")
+    if len(params) != 12 + 2 * (spec.add_fc - 1):
+        raise _lib.Ta3nError(f"the avgpool path takes 12 parameter tensors + 2 per stacked shared layer, "
+                             f"got {len(params)} at add_fc={spec.add_fc}")
     Bs, Bt, D = xs.shape[0], xt.shape[0], xs.shape[2]
     M = Bs + Bt
-    w_sh, b_sh, w1f, b1f, w2f, b2f, w_c, b_c, w1v, b1v, w2v, b2v = params
+    w_sh, b_sh, w1f, b1f, w2f, b2f, w_c, b_c, w1v, b1v, w2v, b2v = params[:12]
     F, Cn = w_sh.shape[0], w_c.shape[0]
     if tuple(w_c.shape) != (Cn, F) or tuple(w1v.shape) != (F, F) or tuple(w2v.shape) != (2, F):
         raise _lib.Ta3nError("avgpool: the video-level layers must be shared_dim wide (models.py:240-250)")
     new = bufs.get
-    d_i, d_v = spec.drop_i.cstruct(), spec.drop_v.cstruct()
-    feat = new("feat", M * T, F)
-    check(lib.ta3n_shared_fc_fwd(_p(xs), Bs * T, _p(xt), Bt * T, D, _p(w_sh), _p(b_sh), F, _dref(d_i), _p(feat), st))
+    d_v = spec.drop_v.cstruct()
+    feats = shared_stack_forward(spec, xs, xt, w_sh, b_sh, _stack_params(params, 12, spec.add_fc), bufs)
+    feat = feats[-1]
     hid_f = pred_frame = None
     if spec.use_attn or not stop_at_video_feature:
         hid_f, pred_frame = new("hid_f", M * T, F), new("pred_frame", M * T, 2)
@@ -530,16 +637,17 @@ def avgpool_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, stop_at_video
     feat_video = new("feat_video", M, F)
     check(lib.ta3n_segment_mean_fwd(_p(feat_att), M, T, F, _p(feat_video), st))
     if stop_at_video_feature:
-        saved = dict(feat=feat, hid_f=hid_f, pred_frame=pred_frame, dropped=None, hid_v=None)
+        saved = dict(feat=feat, hid_f=hid_f, pred_frame=pred_frame, dropped=None, hid_v=None, **_stack_saved(feats))
         outputs = (feat.view(M, T, F), None if pred_frame is None else pred_frame.view(M, T, 2), feat_video, None,
-                   None, None)
+                   None, None) + _stack_outputs(feats, M, T, F)
         return saved, outputs, (Bs, Bt, D, T, F, Cn)
     dropped, pred_video = new("dropped", M, F), new("pred_video", M, Cn)
     check(lib.ta3n_video_head_fwd(_p(feat_video), M, F, Cn, _p(w_c), _p(b_c), _dref(d_v), _p(dropped), _p(pred_video), st))
     hid_v, pred_dom_video = new("hid_v", M, F), new("pred_dom_video", M, 2)
     check(lib.ta3n_disc_fwd(_p(dropped), M, F, F, _p(w1v), _p(b1v), _p(w2v), _p(b2v), _p(hid_v), _p(pred_dom_video), st))
-    saved = dict(feat=feat, hid_f=hid_f, pred_frame=pred_frame, dropped=dropped, hid_v=hid_v)
-    outputs = (feat.view(M, T, F), pred_frame.view(M, T, 2), feat_video, pred_video, pred_dom_video, dropped)
+    saved = dict(feat=feat, hid_f=hid_f, pred_frame=pred_frame, dropped=dropped, hid_v=hid_v, **_stack_saved(feats))
+    outputs = (feat.view(M, T, F), pred_frame.view(M, T, 2), feat_video, pred_video, pred_dom_video,
+               dropped) + _stack_outputs(feats, M, T, F)
     return saved, outputs, (Bs, Bt, D, T, F, Cn)
 
 
@@ -549,8 +657,8 @@ def avgpool_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, buf
     st = _stream()
     Bs, Bt, D, T, F, Cn = dims
     M = Bs + Bt
-    w_sh, b_sh, w1f, b1f, w2f, b2f, w_c, b_c, w1v, b1v, w2v, b2v = params
-    dw_sh, db_sh, dw1f, db1f, dw2f, db2f, dw_c, db_c, dw1v, db1v, dw2v, db2v = gout
+    w_sh, b_sh, w1f, b1f, w2f, b2f, w_c, b_c, w1v, b1v, w2v, b2v = params[:12]
+    dw_sh, db_sh, dw1f, db1f, dw2f, db2f, dw_c, db_c, dw1v, db1v, dw2v, db2v = gout[:12]
     g = lambda k: gin.get(k)   # noqa: E731
     new, wsp = bufs.get, bufs.workspace
     d_v = spec.drop_v.cstruct()
@@ -589,18 +697,15 @@ def avgpool_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, buf
     ws = wsp("disc_f", lib.ta3n_disc_bwd_workspace_bytes(M * T, F, F))
     check(lib.ta3n_disc_bwd(_p(feat), M * T, F, F, _p(w1f), _p(w2f), _p(hid_f), _p(g_pf), float(spec.beta[2]),
                             _p(d_feat), 1, _p(dw1f), _p(db1f), _p(dw2f), _p(db2f), _p(ws), ws.numel(), st))
-    # shared layer (weight gradient only)
-    ws = wsp("shared", lib.ta3n_shared_fc_bwd_workspace_bytes(M * T, D, F))
-    g_feat = g("feat")
-    g_feat_flat = None if g_feat is None else g_feat.reshape(M * T, F)
-    check(lib.ta3n_shared_fc_bwd(_p(xs), Bs * T, _p(xt), Bt * T, D, F, _p(feat), _p(d_feat), _p(g_feat_flat),
-                                 float(spec.drop_i.p), _p(dw_sh), _p(db_sh), _p(ws), ws.numel(), st))
+    # shared layers L..1
+    shared_stack_backward(spec, xs, xt, w_sh, _stack_params(params, 12, spec.add_fc), saved, d_feat, gin, dw_sh, db_sh,
+                          _stack_params(gout, 12, spec.add_fc), bufs)
 
 
 class _AvgPoolPathFunction(torch.autograd.Function):
     """VideoModel.forward with frame_aggregation='avgpool', source and target rows together, as ONE autograd node.
     Outputs (M = Bs + Bt rows, source first): feat_fc (M,T,F) | pred_frame (M,T,2) | feat_video (M,F) |
-    pred_video (M,C) | pred_dom_video (M,2) | dropped (M,F)."""
+    pred_video (M,C) | pred_dom_video (M,2) | dropped (M,F) | feat_fc of the lower shared layers, as in video_path."""
 
     @staticmethod
     def forward(ctx, spec: PathSpec, xs, xt, *params):
@@ -609,7 +714,8 @@ class _AvgPoolPathFunction(torch.autograd.Function):
         saved, outputs, dims = avgpool_forward(spec, xs, xt, params, Buffers(xs.device))
         ctx.spec, ctx.dims = spec, dims
         ctx.saved_names = list(saved)
-        ctx.drop_keepalive = (spec.drop_i.keep, spec.drop_v.keep, spec.drop_i.step, spec.drop_v.step)
+        ctx.out_names = _AVG_OUT_NAMES + _stack_out_names(len(outputs) - len(_AVG_OUT_NAMES))
+        ctx.drop_keepalive = _drop_keepalive(spec)
         ctx.save_for_backward(xs, xt, *[saved[k] for k in ctx.saved_names], *params)
         ctx.set_materialize_grads(False)
         return outputs
@@ -623,7 +729,7 @@ class _AvgPoolPathFunction(torch.autograd.Function):
         n = len(ctx.saved_names)
         saved = dict(zip(ctx.saved_names, tensors[2:2 + n]))
         params = list(tensors[2 + n:])
-        gin = {k: _chk(g, "grad") for k, g in zip(_AVG_OUT_NAMES, grads) if g is not None}
+        gin = {k: _chk(g, "grad") for k, g in zip(ctx.out_names, grads) if g is not None}
         gout = [torch.empty_like(p) for p in params]
         avgpool_backward(ctx.spec, ctx.dims, xs, xt, params, saved, gin, gout, Buffers(xs.device))
         return (None, None, None, *gout)

@@ -59,8 +59,8 @@ class VideoModel(nn.Module):
                          [('avgpool', 'TransAttn', 'none'), ('avgpool', 'none', 'none')])
         if baseline_type != 'video':
             _unsupported('baseline_type', baseline_type, ['video'])
-        if add_fc != 1:
-            _unsupported('add_fc', add_fc, [1])
+        if add_fc > 3:
+            _unsupported('add_fc', add_fc, [1, 2, 3])                     # models.py:145-153: three shared layers at most
         if use_bn != 'none':
             _unsupported('use_bn', use_bn, ['none'])
         if ens_DA not in ('none', 'MCD'):
@@ -105,7 +105,8 @@ class VideoModel(nn.Module):
 
         self._prepare_DA(num_class, base_model)
         self._enable_pbn = partial_bn
-        # test hook: dict with uint8 keep masks 'i' (M*T,F) and 'v' (M,H) overriding the RNG
+        # test hook: dict with uint8 keep masks 'i' (M*T,F) and 'v' (M,H) overriding the RNG; 'i2' / 'i3' (M*T,F) for
+        # the stacked shared layers of add_fc 2 and 3 ('i' is layer 1)
         self.dropout_masks = None
         self._rng = random.Random(0x7A3B200)
 
@@ -128,6 +129,10 @@ class VideoModel(nn.Module):
             return lin
 
         self.fc_feature_shared_source = std_linear(self.feature_dim, feat_shared_dim)   # :141
+        if self.add_fc > 1:
+            self.fc_feature_shared_2_source = std_linear(feat_shared_dim, feat_shared_dim)  # :145-148
+        if self.add_fc > 2:
+            self.fc_feature_shared_3_source = std_linear(feat_shared_dim, feat_shared_dim)  # :150-153
         self.fc_feature_source = std_linear(feat_shared_dim, feat_frame_dim)            # :156 (unused on path)
         self.fc_feature_domain = std_linear(feat_shared_dim, feat_frame_dim)            # :161
         self.fc_classifier_source = std_linear(feat_frame_dim, num_class)               # :166 (output dropped)
@@ -184,21 +189,26 @@ class VideoModel(nn.Module):
         return 1 - torch.sum(-q * torch.log_softmax(pred_domain, dim=1), 1)
 
     def path_parameters(self):
-        """Parameters consumed by the fused operator, in its expected order."""
+        """Parameters consumed by the fused operator, in its expected order; the stacked shared layers of add_fc > 1
+        (W_2, b_2[, W_3, b_3]) come last."""
         if self.frame_aggregation == 'avgpool':
             return [self.fc_feature_shared_source.weight, self.fc_feature_shared_source.bias,
                     self.fc_feature_domain.weight, self.fc_feature_domain.bias,
                     self.fc_classifier_domain.weight, self.fc_classifier_domain.bias,
                     self.fc_classifier_video_source.weight, self.fc_classifier_video_source.bias,
                     self.fc_feature_domain_video.weight, self.fc_feature_domain_video.bias,
-                    self.fc_classifier_domain_video.weight, self.fc_classifier_domain_video.bias]
+                    self.fc_classifier_domain_video.weight, self.fc_classifier_domain_video.bias] + self._stack_parameters()
         R = self.train_segments - 1
         trn_w, trn_b = self.TRN.relation_weights()
         rel = self.relation_domain_classifier_all
         extra = []
         if self.use_attn == 'general':
             extra = [self.attn_layer[0].weight, self.attn_layer[0].bias, self.attn_layer[2].weight, self.attn_layer[2].bias]
-        return self._core_parameters(R, trn_w, trn_b, rel) + extra
+        return self._core_parameters(R, trn_w, trn_b, rel) + extra + self._stack_parameters()
+
+    def _stack_parameters(self):
+        layers = [getattr(self, f'fc_feature_shared_{layer}_source') for layer in range(2, self.add_fc + 1)]
+        return [t for lin in layers for t in (lin.weight, lin.bias)]
 
     def _core_parameters(self, R, trn_w, trn_b, rel):
         return [self.fc_feature_shared_source.weight, self.fc_feature_shared_source.bias,
@@ -212,8 +222,10 @@ class VideoModel(nn.Module):
                 self.fc_classifier_domain_video.weight, self.fc_classifier_domain_video.bias]
 
     def _drop_specs(self, device):
+        """dropout_i of layer 1, dropout_v, and dropout_i of the stacked shared layers (each its own seed, drawn after
+        the other two so that add_fc=1 draws what it always drew)."""
         if not self.training:
-            return TF.DropSpec(), TF.DropSpec()
+            return TF.DropSpec(), TF.DropSpec(), ()
         masks = self.dropout_masks or {}
 
         def spec(p, key):
@@ -226,7 +238,8 @@ class VideoModel(nn.Module):
                 keep = keep.to(device=device, dtype=torch.uint8).contiguous()
             return TF.DropSpec(p=float(p), keep=keep, seed=self._rng.getrandbits(63))
 
-        return spec(self.dropout_rate_i, 'i'), spec(self.dropout_rate_v, 'v')
+        d_i, d_v = spec(self.dropout_rate_i, 'i'), spec(self.dropout_rate_v, 'v')
+        return d_i, d_v, tuple(spec(self.dropout_rate_i, f'i{layer}') for layer in range(2, self.add_fc + 1))
 
     # ---- forward (models.py:545-722) -----------------------------------------------------------------
     def forward(self, input_source, input_target, beta, mu, is_train, reverse):
@@ -244,11 +257,12 @@ class VideoModel(nn.Module):
         xs = xs.reshape(-1, num_segments, xs.size(-1))
         xt = xt.reshape(-1, num_segments, xt.size(-1))
         Bs = xs.size(0)
-        drop_i, drop_v = self._drop_specs(dev)
+        drop_i, drop_v, drop_stack = self._drop_specs(dev)
         spec = TF.PathSpec(num_segments=num_segments, beta=(float(beta[0]), float(beta[1]), float(beta[2])),
                            mu=float(mu), reverse=bool(reverse), use_attn=self.use_attn != 'none',
-                           general_attn=self.use_attn == 'general', use_attn_frame=self.use_attn_frame != 'none', drop_i=drop_i, drop_v=drop_v)
-        feat_fc, pred_frame, attn, pred_rel, feat_video, pred_video, pred_dom_video, dropped = TF.video_path(
+                           general_attn=self.use_attn == 'general', use_attn_frame=self.use_attn_frame != 'none', drop_i=drop_i, drop_v=drop_v,
+                           add_fc=self.add_fc, drop_stack=drop_stack)
+        feat_fc, pred_frame, attn, pred_rel, feat_video, pred_video, pred_dom_video, dropped, *lower = TF.video_path(
             spec, xs, xt, self.path_parameters())
         pred_video_2 = pred_video                                                     # :713-714 out_2 = out
         if self.ens_DA == 'MCD':                                                      # :716-720 (share_params == 'Y')
@@ -264,10 +278,12 @@ class VideoModel(nn.Module):
         out2_s, out2_t = halves(pred_video_2)
         (ff_s, ff_t), (fv_s, fv_t) = halves(feat_fc), halves(feat_video)
         (pf_s, pf_t), (pv_s, pv_t), (pr_s, pr_t) = halves(pred_frame), halves(pred_dom_video), halves(pred_rel)
+        lower_s, lower_t = [t[:Bs] for t in lower], [t[Bs:] for t in lower]
         # lists are returned reversed, as the reference does (models.py:722):
-        #   pred_domain = [relation (B,R,2), video (B,2), frame (B,T,2)];  feat = [pred (B,C), video (B,H), fc (B,T,F)]
-        return (attn_s, out_s, out2_s, [pr_s, pv_s, pf_s], [out_s, fv_s, ff_s],
-                attn_t, out_t, out2_t, [pr_t, pv_t, pf_t], [out_t, fv_t, ff_t])
+        #   pred_domain = [relation (B,R,2), video (B,2), frame (B,T,2)];
+        #   feat = [pred (B,C), video (B,H), fc_L (B,T,F), ..., fc_1 (B,T,F)]   (one fc per shared layer, :578-603)
+        return (attn_s, out_s, out2_s, [pr_s, pv_s, pf_s], [out_s, fv_s, ff_s, *lower_s],
+                attn_t, out_t, out2_t, [pr_t, pv_t, pf_t], [out_t, fv_t, ff_t, *lower_t])
 
     def _forward_avgpool(self, input_source, input_target, beta, mu, num_segments, reverse):
         """frame_aggregation='avgpool' (models.py:620-626, 425-433): no relation level.  The reference fills the relation
@@ -281,11 +297,11 @@ class VideoModel(nn.Module):
         xs = xs.reshape(-1, num_segments, xs.size(-1))
         xt = xt.reshape(-1, num_segments, xt.size(-1))
         Bs = xs.size(0)
-        drop_i, drop_v = self._drop_specs(dev)
+        drop_i, drop_v, drop_stack = self._drop_specs(dev)
         spec = TF.PathSpec(num_segments=num_segments, beta=(float(beta[0]), float(beta[1]), float(beta[2])),
                            mu=float(mu), reverse=bool(reverse), use_attn=self.use_attn == 'TransAttn',
-                           drop_i=drop_i, drop_v=drop_v)
-        feat_fc, pred_frame, feat_video, pred_video, pred_dom_video, dropped = TF.avgpool_path(
+                           drop_i=drop_i, drop_v=drop_v, add_fc=self.add_fc, drop_stack=drop_stack)
+        feat_fc, pred_frame, feat_video, pred_video, pred_dom_video, dropped, *lower = TF.avgpool_path(
             spec, xs, xt, self.path_parameters())
         pred_video_2 = pred_video
         if self.ens_DA == 'MCD':
@@ -298,5 +314,6 @@ class VideoModel(nn.Module):
         (out_s, out_t), (out2_s, out2_t) = halves(pred_video), halves(pred_video_2)
         (ff_s, ff_t), (fv_s, fv_t) = halves(feat_fc), halves(feat_video)
         (pf_s, pf_t), (pv_s, pv_t) = halves(pred_frame), halves(pred_dom_video)
-        return (fv_s[:, 0], out_s, out2_s, [pv_s, pv_s, pf_s], [out_s, fv_s, ff_s],
-                fv_t[:, 0], out_t, out2_t, [pv_t, pv_t, pf_t], [out_t, fv_t, ff_t])
+        lower_s, lower_t = [t[:Bs] for t in lower], [t[Bs:] for t in lower]
+        return (fv_s[:, 0], out_s, out2_s, [pv_s, pv_s, pf_s], [out_s, fv_s, ff_s, *lower_s],
+                fv_t[:, 0], out_t, out2_t, [pv_t, pv_t, pf_t], [out_t, fv_t, ff_t, *lower_t])

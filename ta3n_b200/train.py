@@ -39,6 +39,12 @@ _P = TF._p
 _N_LATE = 6     # path_parameters()[0:6] = shared layer W,b + frame discriminator W1,b1,W2,b2: produced last
 _ALIGN = 64     # floats: every tensor of a flat buffer starts 256-byte aligned (vector stores, TMA operands)
 _PASS2_KEY = 0x6A09E667F3BCC908     # seed of MCD's second pass = step seed ^ this (its masks differ from pass 1's)
+_STACK_KEY = 0xBB67AE8584CAA73B     # dropout seed of stacked shared layer l (add_fc > 1) = pass seed ^ (l - 1) * this
+
+
+def stack_seed(seed: int, layer: int) -> int:
+    """The dropout seed of stacked shared layer ``layer`` (2 or 3) of a pass whose dropout_i seed is ``seed``."""
+    return (int(seed) ^ ((layer - 1) * _STACK_KEY)) & (2 ** 63 - 1)
 
 
 @dataclass
@@ -163,18 +169,33 @@ def step_parameters(model):
     return params
 
 
-def bucket_layout(params):
+def stack_slots(model) -> List[int]:
+    """Indices in ``step_parameters(model)`` of the stacked shared layers' tensors (add_fc > 1): W_2, b_2[, W_3, b_3],
+    the last entries of ``path_parameters()``."""
+    n_path = len(model.path_parameters())
+    return list(range(n_path - 2 * (int(getattr(model, "add_fc", 1)) - 1), n_path))
+
+
+def bucket_layout(params, stack: Sequence[int] = ()):
     """Order and offsets (in floats) of the path's tensors inside a flat buffer: the order in which the
     backward finishes their gradients, [video head, video disc, relation discs, TRN | frame disc, shared layer],
-    every slot padded to ``_ALIGN`` floats.  Returns (order, offsets-by-index, total, early_total)."""
-    order = list(range(_N_LATE, len(params))) + list(range(_N_LATE))
+    every slot padded to ``_ALIGN`` floats.  ``stack`` (``stack_slots``): the stacked shared layers' tensors, which go
+    to the late part too, in completion order [frame disc, shared_3, shared_2, shared_1].
+    Returns (order, offsets-by-index, total, early_total)."""
+    stack = list(stack)
+    early_order = [i for i in range(_N_LATE, len(params)) if i not in stack]
+    if stack:
+        pairs = [stack[i:i + 2] for i in range(0, len(stack), 2)]
+        late = list(range(2, _N_LATE)) + [i for pair in reversed(pairs) for i in pair] + [0, 1]
+    else:
+        late = list(range(_N_LATE))
     offs, off, early = {}, 0, 0
-    for idx in order:
+    for idx in early_order + late:
         offs[idx] = off
         off += -(-params[idx].numel() // _ALIGN) * _ALIGN
-        if idx == len(params) - 1:
+        if idx == early_order[-1]:
             early = off
-    return order, offs, off, early
+    return early_order + late, offs, off, early
 
 
 def flatten_parameters(model) -> torch.Tensor:
@@ -182,7 +203,7 @@ def flatten_parameters(model) -> torch.Tensor:
     that the optimizer is a single pass over contiguous memory.  Values are preserved; idempotent.  The
     Parameter objects (and hence state_dict / load_state_dict / checkpoints) are unchanged."""
     params = step_parameters(model)
-    order, offs, total, _ = bucket_layout(params)
+    order, offs, total, _ = bucket_layout(params, stack_slots(model))
     flat = getattr(model, "_ta3n_flat_params", None)
     if (flat is not None and flat.numel() == total and flat.device == params[0].device and
             all(params[i].data_ptr() == flat.data_ptr() + 4 * offs[i] for i in order)):
@@ -215,7 +236,7 @@ def _updated_slots(model, active: Optional[torch.Tensor]):
     update touches (``active`` is the per-element mask of the update, None = all).  Parameters are matched by identity,
     so MCD's second classifier, appended to the flat buffers, gets its index in ``model.parameters()``."""
     params = step_parameters(model)
-    _, offs, _, _ = bucket_layout(params)
+    _, offs, _, _ = bucket_layout(params, stack_slots(model))
     index = {id(p): i for i, p in enumerate(model.parameters())}
     on = [True] * len(params) if active is None else \
         (active[torch.tensor([offs[j] for j in range(len(params))], device=active.device)] != 0).tolist()
@@ -414,6 +435,18 @@ class TrainStep:
             raise NotImplementedError("TrainStep covers frame_aggregation='trn-m', use_attn in ('TransAttn', 'none') and "
                                       "ens_DA in ('none', 'MCD'); train the other variants with model(...) + "
                                       "loss.backward()")
+        self.add_fc = int(getattr(model, "add_fc", 1))
+        if self.add_fc > 1:
+            # the step program (phased) and what only it carries -- class / domain weights, the DANN beta schedule --
+            # do not cover the stacked shared layers; refused rather than run on another executor
+            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
+                raise NotImplementedError("add_fc > 1 runs in mode='legacy' only (the step program has one shared "
+                                          "layer)")
+            if class_weight is not None or any(float(b) < 0 for b in beta) or \
+                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
+                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
+                                          "(mode='phased'), which does not cover add_fc > 1")
+            mode = "legacy"
         self.mcd = ens == "MCD"
         self.mu = float(mu)
         if self.mu != 0.0 and not self.mcd:
@@ -428,6 +461,7 @@ class TrainStep:
             mode = "legacy"
         self.model = model
         self.params = step_parameters(model)
+        self.n_path = len(model.path_parameters())     # the path operators' tensors; MCD's second classifier follows
         dev = self.params[0].device
         if dev.type != "cuda":
             raise _lib.Ta3nError("TrainStep needs the model on a CUDA device; there is no CPU path")
@@ -494,7 +528,7 @@ class TrainStep:
         #   [ video head, video disc, relation discs, TRN | frame disc, shared layer ]
         # views are installed as .grad; the parameters live in a twin flat buffer (same offsets)
         self.flat_param = flatten_parameters(model)
-        order, offs, n, self.early_numel = bucket_layout(self.params)
+        order, offs, n, self.early_numel = bucket_layout(self.params, stack_slots(model))
         self.flat_grad = self._alloc_gradient_bucket(n, allreduce)
         if self.ar is not None and overlap_allreduce is None:
             self.split = False      # the library's own all-reduce runs inside the one graph: nothing to split around
@@ -579,7 +613,8 @@ class TrainStep:
             num_segments=self.T, beta=tuple(max(b, 0.0) for b in self.beta_spec), mu=0.0, reverse=False,
             use_attn=model.use_attn != "none", use_attn_frame=model.use_attn_frame != "none",
             drop_i=TF.DropSpec(p=di, seed=seed, step=self.step_counter) if di > 0 else TF.DropSpec(),
-            drop_v=TF.DropSpec(p=dv, seed=seed ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec())
+            drop_v=TF.DropSpec(p=dv, seed=seed ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec(),
+            add_fc=self.add_fc, drop_stack=self._stack_drops(seed, di))
         if self.mcd:
             self._init_mcd(seed, di, dv, offs)
         self._init_stats(stats, stats_topk)
@@ -674,6 +709,13 @@ class TrainStep:
         self._need_stats("reset_stats")
         self.stats_acc.zero_()
 
+    def _stack_drops(self, seed, di):
+        """dropout_i of the stacked shared layers: one seed per layer (``stack_seed``), the step counter as key."""
+        if di <= 0:
+            return ()
+        return tuple(TF.DropSpec(p=di, seed=stack_seed(seed, layer), step=self.step_counter)
+                     for layer in range(2, self.add_fc + 1))
+
     def _init_mcd(self, seed, di, dv, offs):
         """State of MCD's second pass: its dropout seeds, buffers, and a second gradient bucket with the bucket's
         layout.  Pass 2 writes its parameter gradients there (every backward entry writes, none accumulates) and one
@@ -688,7 +730,8 @@ class TrainStep:
             num_segments=self.T, beta=self.spec.beta, mu=self.mu, reverse=True, use_attn=self.spec.use_attn,
             use_attn_frame=self.spec.use_attn_frame, classify_only=True,
             drop_i=TF.DropSpec(p=di, seed=s2, step=self.step_counter) if di > 0 else TF.DropSpec(),
-            drop_v=TF.DropSpec(p=dv, seed=s2 ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec())
+            drop_v=TF.DropSpec(p=dv, seed=s2 ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec(),
+            add_fc=self.add_fc, drop_stack=self._stack_drops(s2, di))
         self.bufs2 = TF.Buffers(dev, persistent=True)
         self.x_none = torch.zeros(0, self.T, self.D, **f32)            # pass 2 has no source half
         # pass 2 writes its first classifier's logits over the target rows of pass 1's: those rows of pass 1 feed no
@@ -701,12 +744,12 @@ class TrainStep:
         self.g_video_t, self.g_video2_t = torch.zeros(Bt, C, **f32), torch.zeros(Bt, C, **f32)
         self.flat_grad2 = torch.zeros_like(self.flat_grad)
         self.grad_views2 = [self.flat_grad2[offs[i]:offs[i] + p.numel()].view_as(p) for i, p in enumerate(self.params)]
-        cls = len(self.params) - 8                   # fc_classifier_video_source.weight (then bias, video disc, head 2)
+        cls = 6 + 6 * self.R                         # fc_classifier_video_source.weight (then bias, video disc, head 2)
         self.acc_range = (offs[cls], self.early_numel) if self.mu == 0.0 else (0, self.flat_grad.numel())
 
     def _enqueue_mcd_pass2_forward(self, lib, st):
         """Pass 2's forward (target rows only, fresh masks) and its second classifier."""
-        saved2, out2, dims2 = TF.path_forward(self.spec2, self.x_none, self.xt, self.params, self.bufs2,
+        saved2, out2, dims2 = TF.path_forward(self.spec2, self.x_none, self.xt, self.params[:self.n_path], self.bufs2,
                                               batch_gemms=True)
         w2, b2 = self.params[-2], self.params[-1]
         check(lib.ta3n_video_head_fwd(_P(saved2["dropped"]), self.Bt, w2.shape[1], self.C, _P(w2), _P(b2), None,
@@ -731,8 +774,8 @@ class TrainStep:
         gin = {"pred_video": self.g_video_t}
         if d_dropped is not None:
             gin["dropped"] = d_dropped
-        TF.path_backward(self.spec2, dims2, self.x_none, self.xt, self.params, saved2, gin, self.grad_views2,
-                         self.bufs2)
+        TF.path_backward(self.spec2, dims2, self.x_none, self.xt, self.params[:self.n_path], saved2, gin,
+                         self.grad_views2[:self.n_path], self.bufs2)
         ws = self.bufs2.workspace("wgrad", lib.ta3n_wgrad_defer_workspace_bytes())
         check(lib.ta3n_wgrad_defer_flush(_P(ws), ws.numel(), st))
         lo, hi = self.acc_range
@@ -985,9 +1028,10 @@ class TrainStep:
             self._join_stats()
             return
         check(lib.ta3n_counter_inc(_P(self.step_counter), st))          # fresh dropout masks per step
-        saved, outputs, dims = TF.path_forward(self.spec, self.xs, self.xt, self.params, self.bufs, batch_gemms=True)
+        saved, outputs, dims = TF.path_forward(self.spec, self.xs, self.xt, self.params[:self.n_path], self.bufs,
+                                               batch_gemms=True)
         self.outputs = outputs
-        _, pred_frame, _, pred_rel, _, pred_video, pred_dom, _ = outputs
+        _, pred_frame, _, pred_rel, _, pred_video, pred_dom, _ = outputs[:8]
         if self.mcd:
             # second classifier on the source rows (its target logits of this pass feed no loss), then pass 2's forward
             w2, b2 = self.params[-2], self.params[-1]
@@ -1055,8 +1099,8 @@ class TrainStep:
             self._enqueue_head2_bwd(lib, st, self.bufs, saved["dropped"], self.M, self.g_video2, d_dropped,
                                     self.grad_views)
             gin["dropped"] = d_dropped
-        TF.path_backward(self.spec, dims, self.xs, self.xt, self.params, saved, gin, self.grad_views, self.bufs,
-                         stage_done=stage_done, side_stream=self.branch_stream)
+        TF.path_backward(self.spec, dims, self.xs, self.xt, self.params[:self.n_path], saved, gin,
+                         self.grad_views[:self.n_path], self.bufs, stage_done=stage_done, side_stream=self.branch_stream)
         if self.overlap_wgrad:
             main.wait_stream(side)            # join
         if self.mcd:
