@@ -288,6 +288,30 @@ int ta3n_mcd_loss_fwd_bwd(const float* pred1, const float* pred2, int rows, int 
 /* dst[i] += src[i] for n floats (both 16-byte aligned): sums the gradient buckets of two backward passes.          */
 int ta3n_accumulate(float* dst, const float* src, long long n, ta3n_stream_t stream);
 
+/* ---- discrepancy-based alignment, dis_DA 'DAN' / 'JAN' (main.py:455-505; loss.py:46-120) --------------------- */
+/* Multi-kernel MMD (mmd_rbf, ver 2, fix_sigma None) of up to two layers, or JAN's joint kernel over both, with the
+ * gradient of alpha times the term.  Layer l: source rows xs_l and target rows xt_l ([rows, d_l], contiguous), a
+ * Gaussian kernel sum of num_l bandwidths bw * mul_l^k (bw = the mean off-diagonal squared distance of the rows,
+ * / mul_l^(num_l/2), no gradient through it); xs_l == NULL turns layer l off.  n = min(real source rows, real target
+ * rows) of valid_rows (device {vs, vt}, clamped to Bs / Bt; NULL: Bs / Bt); both sides use their first n rows.
+ *   joint == 0 (DAN): each layer is a level; its n rows are cut into chunks of s = min(256, n) rows, each chunk with
+ *     its own bandwidth, and the level is the mean over its chunks; loss_d = the sum over the levels.  An n above 256
+ *     that 256 does not divide has no chunking in the reference: the term is then 0.
+ *   joint == 1: one chunk of n rows whose kernel is the product of the layers that are on: JAN with both
+ *     (K = K_0 (.) K_1), mmd_rbf without chunks with one.
+ * n == 0 (no real target row) gives 0.  Writes *loss_d = the term, adds alpha * loss_d to *loss (alpha: device
+ * float, NULL = 1; nothing is added when the term is 0), and puts the gradient of alpha * loss_d into gs_l / gt_l:
+ * added to the first n rows (rows past them untouched), or, with bit l of `store`, written there and every other
+ * row of the Bs / Bt rows zeroed.  meter (optional, 3 doubles): {sum += loss_d * vs, last = loss_d, count += vs}.
+ * All sums run in a fixed order (fp64 partials, no atomics): replays are bit-identical.  A chunk whose rows are all
+ * equal has bandwidth 0 and gives NaN, as the reference.  Three launches; no allocation, no synchronisation.   */
+size_t ta3n_discrepancy_workspace_bytes(int Bs, int Bt, int joint);
+int ta3n_discrepancy_fwd_bwd(int joint, int Bs, int Bt,
+                             const float* xs0, const float* xt0, int d0, int num0, float mul0, float* gs0, float* gt0,
+                             const float* xs1, const float* xt1, int d1, int num1, float mul1, float* gs1, float* gt1,
+                             int store, const int* valid_rows, const float* alpha, float* loss, float* loss_d,
+                             double* meter, void* workspace, size_t workspace_bytes, ta3n_stream_t stream);
+
 /* ---- device-resident input pipeline (main.py:343-372 from feature banks in device memory) ---------------------- */
 /* One launch fills the input slot of a paired mini-batch for BOTH domains, for use as the first launch of a captured
  * training step.  Per domain: bank [n_rows, row_floats] fp32 (16-byte aligned; row_floats % 4 == 0), the epoch's row

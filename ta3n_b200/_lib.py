@@ -107,6 +107,9 @@ SIGNATURES = {
     "ta3n_ce_loss_fwd_bwd": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP]),
     "ta3n_mcd_loss_fwd_bwd": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
     "ta3n_accumulate": (_I, [_VP, _VP, C.c_longlong, _VP]),
+    "ta3n_discrepancy_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "ta3n_discrepancy_fwd_bwd": (_I, [_I, _I, _I, _VP, _VP, _I, _I, _F, _VP, _VP, _VP, _VP, _I, _I, _F, _VP, _VP,
+                                      _I, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "ta3n_gather_batch": (_I, [_VP, C.c_longlong, _VP, _VP, C.c_longlong, _I, _VP, _VP,
                                _VP, C.c_longlong, _VP, C.c_longlong, _I, _VP, C.c_longlong, _VP, _VP, _VP]),
     "ta3n_gather_rows": (_I, [_VP, C.c_longlong, _VP, _VP, C.c_longlong, _I, _VP, _VP, C.c_longlong, _VP, _VP, _VP]),

@@ -11,7 +11,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libta3n_sm90.so")
 SOURCES = ["ta3n_api.cu"]
 HEADERS = ["common.cuh", "seg_gemm.cuh", "rowops.cuh", "gemm_wgmma.cuh", "optim.cuh", "step_rows.cuh",
-           "step_plan.cuh", "allreduce.cuh", "gather.cuh", "eval.cuh", "train_stats.cuh",
+           "step_plan.cuh", "allreduce.cuh", "gather.cuh", "eval.cuh", "train_stats.cuh", "discrepancy.cuh",
            os.path.join("..", "..", "include", "ta3n_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

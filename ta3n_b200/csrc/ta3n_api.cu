@@ -11,6 +11,7 @@
 #include "gather.cuh"
 #include "eval.cuh"
 #include "train_stats.cuh"
+#include "discrepancy.cuh"
 
 #include <functional>
 
@@ -1045,6 +1046,72 @@ int ta3n_accumulate(float* dst, const float* src, long long n, ta3n_stream_t str
   TA3N_REQUIRE(aligned16(dst) && aligned16(src), "buffers must be 16-byte aligned");
   pre_launch("accumulate", S(stream));
   launch_kernel(accumulate_kernel, blocks_for((size_t)(n + 3) / 4, 256), 256, 0, S(stream), dst, src, (size_t)n);
+  return after_launch();
+}
+
+// ------------------------------------------------------------------------------------------------
+// discrepancy-based alignment, dis_DA 'DAN' / 'JAN' (main.py:455-505; loss.py:46-120)
+// ------------------------------------------------------------------------------------------------
+size_t ta3n_discrepancy_workspace_bytes(int Bs, int Bt, int joint) {
+  if (Bs < 1 || Bt < 1) return 0;
+  return dis_bytes(dis_geom(Bs, Bt, joint));
+}
+
+int ta3n_discrepancy_fwd_bwd(int joint, int Bs, int Bt,
+                             const float* xs0, const float* xt0, int d0, int num0, float mul0, float* gs0, float* gt0,
+                             const float* xs1, const float* xt1, int d1, int num1, float mul1, float* gs1, float* gt1,
+                             int store, const int* valid_rows, const float* alpha, float* loss, float* loss_d,
+                             double* meter, void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
+  TA3N_REQUIRE(Bs >= 1 && Bt >= 1, "Bs and Bt must be >= 1");
+  TA3N_REQUIRE(xs0 || xs1, "no layer");
+  TA3N_REQUIRE(loss && loss_d, "null loss pointer");
+  DisArgs a;
+  memset(&a, 0, sizeof(a));
+  const float* xs[2] = {xs0, xs1};
+  const float* xt[2] = {xt0, xt1};
+  float* gs[2] = {gs0, gs1};
+  float* gt[2] = {gt0, gt1};
+  const int d[2] = {d0, d1}, num[2] = {num0, num1};
+  const float mul[2] = {mul0, mul1};
+  int dmax = 0;
+  for (int l = 0; l < 2; ++l) {
+    if (!xs[l]) continue;
+    TA3N_REQUIRE(xt[l] && gs[l] && gt[l], "a layer needs source, target and both gradient buffers");
+    TA3N_REQUIRE(d[l] >= 1 && num[l] >= 1 && mul[l] > 0.f, "bad layer width / kernel count / kernel multiplier");
+    TA3N_REQUIRE(gs[l] != gt[l] && (const float*)gs[l] != xs[l] && (const float*)gt[l] != xt[l],
+                 "gradient buffers must not alias each other or the inputs");
+    a.layer[l] = DisLayer{xs[l], xt[l], gs[l], gt[l], d[l], num[l], mul[l], (store >> l) & 1};
+    dmax = std::max(dmax, d[l]);
+  }
+  const DisGeom g = dis_geom(Bs, Bt, joint);
+  TA3N_REQUIRE(workspace && workspace_bytes >= dis_bytes(g), "workspace too small (ta3n_discrepancy_workspace_bytes)");
+  a.joint = joint ? 1 : 0;
+  a.Bs = Bs;
+  a.Bt = Bt;
+  a.cap = g.cap;
+  a.max_chunks = g.max_chunks;
+  a.ntile = g.ntile;
+  a.valid = valid_rows;
+  a.alpha = alpha;
+  a.loss = loss;
+  a.loss_d = loss_d;
+  a.meter = meter;
+  char* w = static_cast<char*>(workspace);
+  a.mats = reinterpret_cast<float*>(w);
+  w += ((g.mats * sizeof(float) + 255) / 256) * 256;
+  a.l2_part = reinterpret_cast<double*>(w);
+  w += ((g.parts * sizeof(double) + 255) / 256) * 256;
+  a.loss_part = reinterpret_cast<double*>(w);
+  const dim3 sq(g.ntile, g.ntile, 2 * g.max_chunks);
+  pre_launch("dis_dist", S(stream));
+  launch_kernel(dis_dist_kernel, sq, kDisThreads, 0, S(stream), a);
+  TA3N_TRY(after_launch());
+  pre_launch("dis_coef", S(stream));
+  launch_kernel(dis_coef_kernel, dim3(g.ntile, g.ntile, joint ? 1 : 2 * g.max_chunks), kDisThreads, 0, S(stream), a);
+  TA3N_TRY(after_launch());
+  pre_launch("dis_grad", S(stream));
+  launch_kernel(dis_grad_kernel, dim3((dmax + kDisTile - 1) / kDisTile, g.ntile, 2 * g.max_chunks), kDisThreads, 0,
+                S(stream), a);
   return after_launch();
 }
 

@@ -773,3 +773,81 @@ class _VideoHead2Function(torch.autograd.Function):
 
 def video_head2(dropped: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor):
     return _VideoHead2Function.apply(dropped, weight, bias)
+
+
+# ----------------------------------------------------------------------------------------------
+# discrepancy-based alignment, dis_DA 'DAN' / 'JAN'             main.py:455-505, loss.py:46-120
+# ----------------------------------------------------------------------------------------------
+DIS_KERNEL_NUMS = (2, 5)     # main.py:458-459: kernel_num of the logits and of the video feature; kernel_mul 2 for both
+
+
+def discrepancy_fwd_bwd(joint: bool, layers, Bs: int, Bt: int, valid, alpha, loss, loss_d, workspace, store: int = 0,
+                        meter=None, stream=None):
+    """One ``ta3n_discrepancy_fwd_bwd`` call (three launches).  ``layers``: two entries, each None (off) or
+    (xs, xt, gs, gt, kernel_num, kernel_mul) with xs / xt the source / target rows [rows, d] and gs / gt their
+    gradient rows.  ``workspace``: at least ``ta3n_discrepancy_workspace_bytes(Bs, Bt, joint)`` bytes."""
+    lib = _lib.load()
+    args = []
+    for lay in layers:
+        if lay is None:
+            args += [None, None, 0, 0, 0.0, None, None]
+            continue
+        xs, xt, gs, gt, num, mul = lay
+        args += [_p(xs), _p(xt), int(xs.shape[-1]), int(num), float(mul), _p(gs), _p(gt)]
+    check(lib.ta3n_discrepancy_fwd_bwd(int(bool(joint)), int(Bs), int(Bt), *args, int(store), _p(valid), _p(alpha),
+                                       _p(loss), _p(loss_d), _p(meter), _p(workspace), workspace.numel(),
+                                       _stream() if stream is None else stream))
+
+
+class _DiscrepancyFunction(torch.autograd.Function):
+    """The term and its input gradients in one call (forward); backward scales the stored gradients."""
+
+    @staticmethod
+    def forward(ctx, joint, nums, muls, *xs_xt):
+        lib = _lib.load()
+        k = len(xs_xt) // 2
+        srcs = [_chk(x, "source") for x in xs_xt[:k]]
+        tgts = [_chk(x, "target") for x in xs_xt[k:]]
+        for s, t in zip(srcs, tgts):
+            if s.dim() != 2 or t.dim() != 2 or s.shape[1] != t.shape[1]:
+                raise _lib.Ta3nError(f"discrepancy: layers must be 2-D with equal widths, got {tuple(s.shape)} / "
+                                     f"{tuple(t.shape)}")
+        # the entry point reads Bs rows of every source layer and Bt of every target layer (and zeroes the gradient
+        # rows past the pairs there): the layers of one domain must agree, as the kernel product of loss.JAN needs
+        Bs, Bt = srcs[0].shape[0], tgts[0].shape[0]
+        if any(s.shape[0] != Bs for s in srcs) or any(t.shape[0] != Bt for t in tgts):
+            raise _lib.Ta3nError(f"discrepancy: the layers of a domain need one row count, got source "
+                                 f"{[s.shape[0] for s in srcs]} / target {[t.shape[0] for t in tgts]}")
+        dev = srcs[0].device
+        if min(Bs, Bt) == 0:
+            ctx.grads = [torch.zeros_like(x) for x in srcs + tgts]
+            return torch.zeros((), device=dev, dtype=torch.float32)
+        gs = [torch.empty_like(s) for s in srcs]
+        gt = [torch.empty_like(t) for t in tgts]
+        layers = [(srcs[i], tgts[i], gs[i], gt[i], nums[i], muls[i]) for i in range(k)] + [None] * (2 - k)
+        loss = torch.zeros(1, device=dev, dtype=torch.float32)
+        loss_d = torch.zeros(1, device=dev, dtype=torch.float32)
+        ws = _ws(lib.ta3n_discrepancy_workspace_bytes(Bs, Bt, int(joint)), srcs[0])
+        discrepancy_fwd_bwd(joint, layers, Bs, Bt, None, None, loss, loss_d, ws, store=(1 << k) - 1)
+        ctx.grads = gs + gt
+        return loss_d[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        return (None, None, None) + tuple(g * t for t in ctx.grads)
+
+
+def mmd_loss(source, target, kernel_mul: float = 2.0, kernel_num: int = 5):
+    """``loss.mmd_rbf(source[:n], target[:n], kernel_mul, kernel_num)`` (ver 2, fix_sigma None) on CUDA, n = the
+    smaller row count, with its gradient; one fused call.  No chunking: this is one DAN chunk of any size."""
+    return _DiscrepancyFunction.apply(True, (int(kernel_num),), (float(kernel_mul),), source, target)
+
+
+def jan_loss(source_list, target_list, kernel_muls=(2.0, 2.0), kernel_nums=DIS_KERNEL_NUMS):
+    """``loss.JAN`` of two layers (ver 2, fix_sigma None) on CUDA over the first n = min(rows) rows of each side, with
+    its gradient; one fused call.  The source layers share one row count, the target layers another (Ta3nError
+    otherwise)."""
+    if len(source_list) != 2 or len(target_list) != 2:
+        raise ValueError("jan_loss takes two layers per domain, as main.py:462-471 passes")
+    return _DiscrepancyFunction.apply(True, tuple(int(k) for k in kernel_nums), tuple(float(m) for m in kernel_muls),
+                                      *source_list, *target_list)

@@ -24,7 +24,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import math
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -33,6 +33,7 @@ import torch.distributed as dist
 
 from . import _lib
 from . import functional as TF
+from . import loss as LS
 from ._lib import check
 
 _P = TF._p
@@ -93,7 +94,8 @@ class TrainStats:
     """The meters of main.py's train() (main.py:311-320) over the steps since the last ``reset_stats()``: ``loss``,
     ``loss_c``, ``loss_a``, ``loss_e``, ``loss_s`` and, per k of ``topk``, the precision meter ``prec[k]`` (percent;
     ``top1`` / ``top5`` when those k are kept).  A meter whose term is switched off keeps count 0.  ``correct`` and
-    ``rows``: the epoch's top-k hits and real source rows; ``steps``: the steps folded in."""
+    ``rows``: the epoch's top-k hits and real source rows; ``steps``: the steps folded in.  ``loss_d``: the
+    discrepancy term without alpha (``losses_d``, main.py:504) under dis_DA 'DAN' / 'JAN', else empty."""
     loss: Meter
     loss_c: Meter
     loss_a: Meter
@@ -104,6 +106,7 @@ class TrainStats:
     correct: Tuple[int, ...]
     rows: int
     steps: int
+    loss_d: Meter = field(default_factory=Meter)
 
     @property
     def top1(self) -> Optional[Meter]:
@@ -137,8 +140,8 @@ def parse_train_stats(words, topk: Sequence[int]) -> TrainStats:
 class TrainStatsSnapshot:
     """``TrainStep.stats_async()``: the accumulator copied to pinned host memory behind an event."""
 
-    def __init__(self, host: torch.Tensor, event, topk: Tuple[int, ...]):
-        self._host, self._event, self._topk = host, event, topk
+    def __init__(self, host: torch.Tensor, event, topk: Tuple[int, ...], dis_host: Optional[torch.Tensor] = None):
+        self._host, self._event, self._topk, self._dis_host = host, event, topk, dis_host
 
     def done(self) -> bool:
         return self._event.query()
@@ -146,7 +149,16 @@ class TrainStatsSnapshot:
     def result(self) -> TrainStats:
         """Wait for the copy (not for later work on the stream) and return the snapshot."""
         self._event.synchronize()
-        return parse_train_stats(self._host.numpy(), self._topk)
+        st = parse_train_stats(self._host.numpy(), self._topk)
+        if self._dis_host is not None:
+            st.loss_d = dis_meter(self._dis_host.numpy())
+        return st
+
+
+def dis_meter(words) -> Meter:
+    """The ``loss_d`` meter from its accumulator {sum of val * n, last val, sum of n} (3 doubles)."""
+    s, val, n = (float(x) for x in words)
+    return Meter(val=val, avg=s / n if n else 0.0, sum=s, count=int(n))
 
 
 def lr_dann(lr0: float, p: float) -> float:
@@ -157,6 +169,18 @@ def lr_dann(lr0: float, p: float) -> float:
 def beta_dann(p: float) -> float:
     """main.py:351: the DANN schedule of the GRL coefficient; replaces every NEGATIVE entry of --beta (main.py:352)."""
     return 2.0 / (1.0 + math.exp(-10.0 * p)) - 1.0
+
+
+def alpha_dann(epoch: int, epochs: int) -> float:
+    """main.py:231: the weight of the discrepancy loss when --alpha is negative, set once per epoch."""
+    return 2.0 / (1.0 + math.exp(-epoch / epochs)) - 1.0
+
+
+def _negative_alpha(alpha):
+    # main.py:231 reads a negative --alpha as "use the schedule", never as a weight: passing it through would maximise
+    # the discrepancy
+    raise ValueError(f"alpha={alpha}: a negative --alpha selects the schedule of main.py:231; pass "
+                     "alpha_dann(epoch, epochs), or set_alpha(alpha_dann(epoch, epochs)) once per epoch")
 
 
 def step_parameters(model):
@@ -370,7 +394,8 @@ class TrainStep:
                  optimizer: Optional[Optimizer] = None, mode: Optional[str] = None,
                  class_weight: Optional[torch.Tensor] = None, domain_weight: Sequence[float] = (1.0, 1.0),
                  allreduce: Optional[str] = None, mu: float = 0.0, sampler=None, stats: bool = False,
-                 stats_topk: Sequence[int] = (1, 5)):
+                 stats_topk: Sequence[int] = (1, 5), dis_DA: str = "none", alpha: float = 0.0,
+                 place_dis: Sequence[str] = ("Y", "Y", "N")):
         """mode: 'legacy' (default) = the per-operator sequence (25 launches in one CUDA graph; the only mode that
         supports use_attn_frame); 'phased' = the step program as 14 launches (ta3n_step_run_phased; default when class /
         domain weights or a scheduled beta are given).  class_weight / domain_weight: the weights of criterion /
@@ -405,7 +430,18 @@ class TrainStep:
         stats: keep the meters of main.py's train() on the device (``ta3n_train_stats_accumulate``, one launch per
         step after the loss launches, in the same graph): the loss, each loss term and the top-k accuracy of
         ``stats_topk`` (one to four k in [1, C]) on the batch's real source rows.  ``stats()`` reads them back,
-        ``stats_async()`` without stalling the stream, ``reset_stats()`` starts an epoch.  Single rank only."""
+        ``stats_async()`` without stalling the stream, ``reset_stats()`` starts an epoch.  Single rank only.
+
+        dis_DA ('DAN' / 'JAN', mode 'legacy', single rank): the discrepancy loss of main.py:455-505 on this pass's
+        video logits (after dropout_v) and video feature (before it), added to the loss as alpha * loss_d
+        (``loss.discrepancy_loss``; three launches after the loss launches, ``ta3n_discrepancy_fwd_bwd``).  DAN takes
+        the levels l with place_dis[l] == 'Y' (0: logits, 1: video feature; the 3-D shared-layer levels are refused, as
+        the reference cannot compute them), JAN both.  Rows: the first min(real source, real target) of each side; a
+        batch with no real target row, or (DAN) a short last batch of more than 256 such rows that 256 does not divide,
+        contributes 0 to the loss and the gradient (the reference fails on both).  Under MCD the term reads pass 1's
+        outputs.  alpha: a device scalar, rescheduled by ``set_alpha`` (``alpha_dann`` per epoch) without re-capture;
+        a negative alpha raises ValueError (main.py:231 reads it as "use the schedule", not as a weight).
+        With stats=True the ``loss`` meter includes alpha * loss_d and ``TrainStats.loss_d`` holds the term."""
         if optimizer is not None and not isinstance(optimizer, (SGDNesterov, Adam)):
             raise TypeError(f"optimizer must be SGDNesterov or Adam, got {type(optimizer).__name__}")
         if isinstance(optimizer, Adam):
@@ -459,6 +495,12 @@ class TrainStep:
                 raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
                                           "(mode='phased'), which does not cover ens_DA='MCD'")
             mode = "legacy"
+        if dis_DA != "none":
+            self._check_dis(dis_DA, alpha, mode, class_weight, beta, domain_weight, process_group, place_dis,
+                            batch_source, batch_target)
+            mode = "legacy"
+        elif float(alpha) != 0.0:
+            raise ValueError("alpha weights the discrepancy loss (dis_DA='DAN' / 'JAN'); without it it does nothing")
         self.model = model
         self.params = step_parameters(model)
         self.n_path = len(model.path_parameters())     # the path operators' tensors; MCD's second classifier follows
@@ -618,6 +660,7 @@ class TrainStep:
         if self.mcd:
             self._init_mcd(seed, di, dv, offs)
         self._init_stats(stats, stats_topk)
+        self._init_dis(dis_DA, alpha, place_dis)
         self.outputs = None
         self.branch_stream = torch.cuda.Stream(device=dev) if parallel_branches else None
         self.overlap_wgrad = bool(overlap_wgrad)
@@ -644,6 +687,71 @@ class TrainStep:
             sampler.rewind()        # the capture's warm-up ran one gather
         if self.keep_stats:
             self.reset_stats()      # and folded one step into the meters
+
+    def _check_dis(self, dis_DA, alpha, mode, class_weight, beta, domain_weight, group, place_dis, Bs, Bt):
+        """The options dis_DA cannot run with (raised at construction, before anything is allocated)."""
+        if dis_DA == "CORAL":
+            raise NotImplementedError("dis_DA='CORAL': main.py:493 calls a CORAL loss that the reference never defines")
+        if dis_DA not in ("DAN", "JAN"):
+            raise ValueError(f"dis_DA must be 'none', 'DAN' or 'JAN', got {dis_DA!r}")
+        if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
+            raise NotImplementedError("dis_DA runs in mode='legacy' only (the step program has no discrepancy loss)")
+        if class_weight is not None or any(float(b) < 0 for b in beta) or \
+                tuple(float(w) for w in domain_weight) != (1.0, 1.0):
+            raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
+                                      "(mode='phased'), which does not cover dis_DA")
+        if (dist.get_world_size(group) if dist.is_initialized() else 1) > 1:
+            # every row is paired with every other row of the batch: an MMD per shard is a different loss
+            raise NotImplementedError("dis_DA runs on a single rank: the MMD pairs rows across the whole batch")
+        if float(alpha) < 0:
+            _negative_alpha(alpha)
+        if dis_DA == "DAN":
+            LS.dis_levels(place_dis, self.add_fc)
+            n = min(int(Bs), int(Bt))
+            if n > LS._DIS_CHUNK and n % LS._DIS_CHUNK:
+                raise ValueError(f"dis_DA='DAN' with min(Bs, Bt) = {n}: above 256 rows the reference cuts the batch "
+                                 "into chunks of 256 and fails unless 256 divides it")
+
+    def _init_dis(self, dis_DA, alpha, place_dis):
+        """Buffers of the discrepancy loss: alpha, the unscaled term, the video feature's gradient, the workspace and
+        (stats) the loss_d meter; under MCD a copy of pass 1's target logits, which pass 2 overwrites."""
+        self.dis_DA = dis_DA
+        if dis_DA == "none":
+            return
+        f32 = dict(device=self.device, dtype=torch.float32)
+        self.dis_joint = dis_DA == "JAN"
+        levels = (0, 1) if self.dis_joint else LS.dis_levels(place_dis, self.add_fc)
+        self.dis_on = (0 in levels, 1 in levels)
+        self.alpha_dev = torch.full((1,), float(alpha), **f32)
+        self.loss_d = torch.zeros(1, **f32)
+        H = self.model.fc_classifier_video_source.weight.shape[1]
+        self.g_feat_video = torch.zeros(self.M, H, **f32) if self.dis_on[1] else None
+        self.pred_video_t1 = torch.zeros(self.Bt, self.C, **f32) if (self.mcd and self.dis_on[0]) else None
+        nbytes = _lib.load().ta3n_discrepancy_workspace_bytes(self.Bs, self.Bt, int(self.dis_joint))
+        self.dis_ws = torch.zeros(max(256, nbytes), device=self.device, dtype=torch.uint8)
+        self.dis_meter = torch.zeros(3, device=self.device, dtype=torch.float64) if self.keep_stats else None
+
+    def _enqueue_dis(self, st, feat_video, pred_video):
+        """alpha * loss_d into the loss; the logits' gradient added to g_video, the video feature's written to
+        g_feat_video (rows past the pairs zeroed), which the backward takes as gin['feat_video']."""
+        Bs, layers = self.Bs, [None, None]
+        if self.dis_on[0]:
+            xt = self.pred_video_t1 if self.pred_video_t1 is not None else pred_video[Bs:]
+            layers[0] = (pred_video[:Bs], xt, self.g_video[:Bs], self.g_video[Bs:], TF.DIS_KERNEL_NUMS[0], 2.0)
+        if self.dis_on[1]:
+            g = self.g_feat_video
+            layers[1] = (feat_video[:Bs], feat_video[Bs:], g[:Bs], g[Bs:], TF.DIS_KERNEL_NUMS[1], 2.0)
+        TF.discrepancy_fwd_bwd(self.dis_joint, layers, Bs, self.Bt, self.valid, self.alpha_dev, self.loss, self.loss_d,
+                               self.dis_ws, store=2, meter=self.dis_meter, stream=st)
+
+    def set_alpha(self, alpha: float):
+        """The weight of the discrepancy loss for the following steps (main.py:231: ``alpha_dann(epoch, epochs)`` when
+        --alpha is negative): one 4-byte fill on the stream, no re-capture."""
+        if self.dis_DA == "none":
+            raise ValueError("set_alpha needs TrainStep(dis_DA='DAN' or 'JAN')")
+        if float(alpha) < 0:
+            _negative_alpha(alpha)
+        self.alpha_dev.fill_(float(alpha))
 
     def _init_stats(self, stats, topk):
         """The meters' accumulator (ta3n_train_stats), its workspace and the launch's host arguments."""
@@ -691,7 +799,10 @@ class TrainStep:
     def stats(self) -> TrainStats:
         """The meters since the last ``reset_stats()`` (one blocking readback on the current stream)."""
         self._need_stats("stats")
-        return parse_train_stats(self.stats_acc.cpu().numpy(), self.stats_topk)
+        st = parse_train_stats(self.stats_acc.cpu().numpy(), self.stats_topk)
+        if self.dis_DA != "none":
+            st.loss_d = dis_meter(self.dis_meter.cpu().numpy())
+        return st
 
     def stats_async(self) -> TrainStatsSnapshot:
         """Copy the meters into pinned host memory behind an event on the current stream and return at once;
@@ -699,15 +810,21 @@ class TrainStep:
         self._need_stats("stats_async")
         host = torch.empty(_STATS_WORDS, dtype=torch.int64, pin_memory=True)
         host.copy_(self.stats_acc, non_blocking=True)
+        dis_host = None
+        if self.dis_DA != "none":
+            dis_host = torch.empty(3, dtype=torch.float64, pin_memory=True)
+            dis_host.copy_(self.dis_meter, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
-        return TrainStatsSnapshot(host, ev, self.stats_topk)
+        return TrainStatsSnapshot(host, ev, self.stats_topk, dis_host)
 
     def reset_stats(self) -> None:
         """Start an epoch of meters (main.py builds fresh AverageMeters in every train() call): zeroes the accumulator
         on the current stream, no re-capture."""
         self._need_stats("reset_stats")
         self.stats_acc.zero_()
+        if self.dis_DA != "none":
+            self.dis_meter.zero_()
 
     def _stack_drops(self, seed, di):
         """dropout_i of the stacked shared layers: one seed per layer (``stack_seed``), the step counter as key."""
@@ -1037,6 +1154,8 @@ class TrainStep:
             w2, b2 = self.params[-2], self.params[-1]
             check(lib.ta3n_video_head_fwd(_P(saved["dropped"]), self.Bs, w2.shape[1], self.C, _P(w2), _P(b2), None,
                                           _P(self.head2_scratch), _P(self.pred2_s), st))
+            if self.dis_DA != "none" and self.pred_video_t1 is not None:
+                self.pred_video_t1.copy_(pred_video[self.Bs:])      # pass 2 writes its target logits over these
             saved2, dims2 = self._enqueue_mcd_pass2_forward(lib, st)
         check(lib.ta3n_loss_fwd_bwd(_P(pred_video), _P(self.labels), _P(pred_rel), _P(pred_dom), _P(pred_frame),
                                     self.Bs, self.Bt, self.T, self.R, self.C, self.gamma, self.flags,
@@ -1049,10 +1168,14 @@ class TrainStep:
             check(lib.ta3n_mcd_loss_fwd_bwd(_P(pred_video[self.Bs:]), _P(self.pred2_t), self.Bt, self.C, _P(self.valid),
                                             _P(self.loss), _P(self.g_video_t), _P(self.g_video2_t),
                                             _P(self.g_video[self.Bs:]), st))
+        if self.dis_DA != "none":
+            self._enqueue_dis(st, outputs[4], pred_video)
         if self.keep_stats:
             self._enqueue_stats(lib, st, pred_video, pred_rel, pred_dom, pred_frame)
         gin = {"pred_video": self.g_video, "pred_rel": self.g_rel, "pred_dom_video": self.g_dom,
                "pred_frame": self.g_frame}
+        if self.dis_DA != "none" and self.g_feat_video is not None:
+            gin["feat_video"] = self.g_feat_video
         # The data-gradient chain runs first; the weight-gradient GEMMs / bias sums it leaves behind are deferred
         # and issued as grouped launches (buffers and workspaces are persistent, so they stay valid):
         #   one batch at the end, or -- split mode -- one after the TRN stage (early bucket) and one at the end.
