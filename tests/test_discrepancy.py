@@ -516,19 +516,19 @@ def test_train_step_matches_fp64_oracle(case, engine):
     if add_fc == 1:
         # the ReLU pattern the step realised (a unit near 0 may flip under tf32x3), flip-bounded as elsewhere
         from tests.test_gpu_parity import FLIP_BOUND
-        from tests.test_mcd_train_step import _realised_gates
+        from tests.pinned_pattern import realised_gates
         ones = lambda r: torch.ones(r, cfg.shared_dim, dtype=torch.bool)              # noqa: E731
         kept = ones((ns + nt) * T) if masks is None else torch.cat([masks["i_source"], masks["i_target"]]).bool()
         frames = lambda t: torch.cat([t[:ns * T], t[Bs * T:Bs * T + nt * T]]).cpu()    # noqa: E731
         videos = lambda t: torch.cat([t[:ns], t[Bs:Bs + nt]]).cpu()                    # noqa: E731
-        gates, flips, total = _realised_gates(step.bufs.pool, frames, videos, kept, gates, True, True)
+        gates, flips, total = realised_gates(step.bufs.pool, frames, videos, kept, gates, True, True)
         if ens == "MCD":
             k2 = None if masks2 is None else {"i_source": torch.ones(0, cfg.shared_dim, dtype=torch.uint8),
                                               "v_source": torch.ones(0, cfg.video_dim, dtype=torch.uint8), **masks2}
             plain2 = orc.activation_pattern(p64, xs[:0].double(), xt.double(), BETA, cfg, masks=k2)
             kept2 = ones(nt * T) if masks2 is None else masks2["i_target"].bool()
-            g2, f2, n2 = _realised_gates(step.bufs2.pool, lambda t: t[:nt * T].cpu(), lambda t: t[:nt].cpu(), kept2,
-                                         plain2, attn_frame != "none", False)
+            g2, f2, n2 = realised_gates(step.bufs2.pool, lambda t: t[:nt * T].cpu(), lambda t: t[:nt].cpu(), kept2,
+                                        plain2, attn_frame != "none", False)
             _, gates2 = orc.split_gates(g2, 0, T)
             flips, total = flips + f2, total + n2
         assert flips <= max(FLIP_BOUND[engine] * total, 2), (flips, total)

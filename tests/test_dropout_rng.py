@@ -18,8 +18,8 @@ import torch
 from oracle import dropout_rng as drng
 from oracle import ta3n_oracle as orc
 from tests.golden_util import abs_err, assert_close
-from tests.test_gpu_parity import (ENGINES, FLIP_BOUND, GRAD_TOL, NOISE_SCALE, PINNED_TOL, TOL, build_model,
-                                   flat_outputs)
+from tests.pinned_pattern import assert_dropped_units_zero, assert_pinned_grads, real_rows, realised_gates
+from tests.test_gpu_parity import ENGINES, FLIP_BOUND, GRAD_TOL, NOISE_SCALE, TOL, build_model, flat_outputs
 
 gpu = pytest.mark.gpu
 
@@ -307,10 +307,6 @@ def _replay_and_key(step, mode, *batch):
     return loss.cpu()[0].clone(), (before + 1 if mode == "legacy" else before)
 
 
-def _gate_list(g):
-    return [g["frame_disc"], *g["trn"], *g["rel_disc"], g["video_disc"]]
-
-
 def _check_step(step, key, loss, cfg, params, xs, xt, labels, beta, engine, what, flip_floor=2):
     """One TrainStep replay (kernels keyed with `key`) against the fp64 oracle on the rebuilt masks of its real rows
     (xs / xt may be a short batch; the captured batch is step.Bs + step.Bt).
@@ -325,34 +321,20 @@ def _check_step(step, key, loss, cfg, params, xs, xt, labels, beta, engine, what
     masks = drng.train_step_masks(key, step.Bs, step.Bt, T, cfg.shared_dim, cfg.video_dim, cfg.dropout_i,
                                   cfg.dropout_v, ns=ns, nt=nt)
     pool = step.bufs.pool
-    frames = lambda t: torch.cat([t[:ns * T], t[step.Bs * T:step.Bs * T + nt * T]]).cpu()    # noqa: E731
-    videos = lambda t: torch.cat([t[:ns], t[step.Bs:step.Bs + nt]]).cpu()                    # noqa: E731
-    feat = frames(pool["feat"])
+    frames, videos = real_rows(step.Bs, ns, nt, T)
     kept = torch.cat([masks["i_source"], masks["i_target"]]).bool()
-    assert torch.all(feat[~kept] == 0), f"{what}: a unit the restated mask drops is nonzero"
     kept_v = torch.cat([masks["v_source"], masks["v_target"]]).bool()
-    assert torch.all(videos(pool["dropped"])[~kept_v] == 0), f"{what}: a video unit the restated mask drops is nonzero"
+    assert_dropped_units_zero(pool, frames, videos, kept, kept_v, what)
     p64 = {k: (v.double() if v.dtype.is_floating_point else v) for k, v in params.items()}
     plain = orc.activation_pattern(p64, xs.double(), xt.double(), beta, cfg, masks=masks)
-    gates = {"shared": torch.where(kept, feat > 0, plain["shared"]), "frame_disc": frames(pool["hid_f"]) > 0,
-             "trn": [videos(a) > 0 for a in pool["act"]], "rel_disc": [videos(h) > 0 for h in pool["hid_r"]],
-             "video_disc": videos(pool["hid_v"]) > 0}
-    flips = ((gates["shared"] != plain["shared"]) & kept).sum().item()
-    total = kept.sum().item()
-    for a, b in zip(_gate_list(gates), _gate_list(plain)):
-        flips += (a != b).sum().item()
-        total += a.numel()
+    gates, flips, total = realised_gates(pool, frames, videos, kept, plain)
     print(f"{what}: {flips} of {total} ReLU units differ from the fp64 pattern")
     assert flips <= max(FLIP_BOUND[engine] * total, flip_floor), (what, flips, total)
     l64, _, g64 = orc.train_step(p64, xs.double(), xt.double(), labels, beta, cfg, 0.003, train=True, masks=masks,
                                  gates=gates)
     l32, _, g32 = orc.train_step(params, xs, xt, labels, beta, cfg, 0.003, train=True, masks=masks, gates=gates)
     assert_close(loss, l64, TOL[engine], f"{what} loss", noise=max(abs(l32.item() - l64.item()), 1e-7))
-    named = dict(step.model.named_parameters())
-    for name, go in g64.items():
-        assert named[name].grad is not None, name
-        assert_close(named[name].grad, go, PINNED_TOL[engine], f"{what} grad {name}",
-                     noise=abs_err(g32[name], go) * NOISE_SCALE[engine])
+    assert_pinned_grads(dict(step.model.named_parameters()), g64, g32, engine, what)
     return masks
 
 

@@ -17,7 +17,8 @@ from oracle import gen_golden_mcd as gen
 from oracle import mcd_oracle as mcd
 from oracle import ref_shims
 from oracle import ta3n_oracle as orc
-from tests.golden_util import TOL_FP32, abs_err, assert_close
+from tests.golden_util import TOL_FP32, assert_close
+from tests.pinned_pattern import assert_dropped_units_zero, assert_pinned_grads, real_rows, realised_gates
 
 gpu = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -202,31 +203,11 @@ def _gpu_case(name, dropout=0.0, seed=5):
     return cfg, params, xs, xt, labels, mu
 
 
-def _gate_list(g):
-    return [g.get("frame_disc"), *g["trn"], *g["rel_disc"], g.get("video_disc")]
-
-
-def _realised_gates(pool, rows_f, rows_v, kept, plain, frame_disc, video_disc):
-    """The step's ReLU pattern in the oracle's gate format (see test_dropout_rng._check_step)."""
-    gates = {"shared": torch.where(kept, rows_f(pool["feat"]) > 0, plain["shared"]),
-             "trn": [rows_v(a) > 0 for a in pool["act"]], "rel_disc": [rows_v(h) > 0 for h in pool["hid_r"]]}
-    if frame_disc:
-        gates["frame_disc"] = rows_f(pool["hid_f"]) > 0
-    if video_disc:
-        gates["video_disc"] = rows_v(pool["hid_v"]) > 0
-    flips = ((gates["shared"] != plain["shared"]) & kept).sum().item()
-    total = kept.sum().item()
-    for a, b in zip(_gate_list(gates), _gate_list(plain)):
-        if a is not None:
-            flips += (a != b).sum().item()
-            total += a.numel()
-    return gates, flips, total
-
-
-def _check_mcd_step(step, key, loss, cfg, params, xs, xt, labels, mu, engine, what):
+def _check_mcd_step(step, key, loss, cfg, params, xs, xt, labels, mu, engine, what, beta=BETA, noise_floor=0.0):
     """One MCD step (kernels keyed with `key`, or no dropout) against the fp64 oracle iteration on the masks both
-    passes drew and the ReLU pattern they realised (flip-bounded as in test_dropout_rng)."""
-    from tests.test_gpu_parity import FLIP_BOUND, NOISE_SCALE, PINNED_TOL, TOL
+    passes drew and the ReLU pattern they realised (flip-bounded as in test_dropout_rng).  Returns the worst gradient
+    error beyond the noise allowance (``noise_floor``: tests.pinned_pattern.assert_pinned_grads)."""
+    from tests.test_gpu_parity import FLIP_BOUND, TOL
     ns, nt, T, Fd, H = xs.shape[0], xt.shape[0], cfg.num_segments, cfg.shared_dim, cfg.video_dim
     m1 = m2 = None
     ones = lambda r, c: torch.ones(r, c, dtype=torch.uint8)      # noqa: E731
@@ -238,33 +219,29 @@ def _check_mcd_step(step, key, loss, cfg, params, xs, xt, labels, mu, engine, wh
         k1 = m1
         k2 = {"i_source": ones(0, Fd), "v_source": ones(0, H), **m2}
     p64 = {k: (v.double() if v.dtype.is_floating_point else v) for k, v in params.items()}
-    frames1 = lambda t: torch.cat([t[:ns * T], t[step.Bs * T:step.Bs * T + nt * T]]).cpu()    # noqa: E731
-    videos1 = lambda t: torch.cat([t[:ns], t[step.Bs:step.Bs + nt]]).cpu()                    # noqa: E731
+    frames1, videos1 = real_rows(step.Bs, ns, nt, T)
+    frames2, videos2 = real_rows(0, 0, nt, T)                    # pass 2 runs the target rows alone
     kept1 = torch.cat([k1["i_source"], k1["i_target"]]).bool()
-    plain1 = orc.activation_pattern(p64, xs.double(), xt.double(), BETA, cfg, masks=m1)
-    g1, f1, n1 = _realised_gates(step.bufs.pool, frames1, videos1, kept1, plain1, True, True)
-    plain2 = orc.activation_pattern(p64, xs[:0].double(), xt.double(), BETA, cfg,
+    plain1 = orc.activation_pattern(p64, xs.double(), xt.double(), beta, cfg, masks=m1)
+    g1, f1, n1 = realised_gates(step.bufs.pool, frames1, videos1, kept1, plain1, True, True)
+    plain2 = orc.activation_pattern(p64, xs[:0].double(), xt.double(), beta, cfg,
                                     masks=None if m2 is None else k2)
     kept2 = k2["i_target"].bool()
     frame_attn = cfg.use_attn_frame != "none"
-    g2, f2, n2 = _realised_gates(step.bufs2.pool, lambda t: t[:nt * T].cpu(), lambda t: t[:nt].cpu(), kept2, plain2,
-                                 frame_attn, False)
+    g2, f2, n2 = realised_gates(step.bufs2.pool, frames2, videos2, kept2, plain2, frame_attn, False)
     print(f"{what}: {f1} + {f2} of {n1} + {n2} ReLU units differ from the fp64 pattern")
     assert f1 + f2 <= max(FLIP_BOUND[engine] * (n1 + n2), 2), (what, f1, f2)
     if m1 is not None:
-        assert torch.all(frames1(step.bufs.pool["feat"])[~kept1] == 0), what
-        assert torch.all(step.bufs2.pool["feat"][:nt * T].cpu()[~kept2] == 0), what
+        assert_dropped_units_zero(step.bufs.pool, frames1, videos1, kept1,
+                                  torch.cat([m1["v_source"], m1["v_target"]]).bool(), what + " pass 1")
+        assert_dropped_units_zero(step.bufs2.pool, frames2, videos2, kept2, m2["v_target"].bool(), what + " pass 2")
     _, gt2 = orc.split_gates(g2, 0, T)
-    l64, _, _, gr64 = mcd.mcd_train_step(p64, xs.double(), xt.double(), labels, BETA, mu, cfg, 0.003, masks=m1,
+    l64, _, _, gr64 = mcd.mcd_train_step(p64, xs.double(), xt.double(), labels, beta, mu, cfg, 0.003, masks=m1,
                                          masks2=m2, gates=g1, gates2=gt2)
-    l32, _, _, gr32 = mcd.mcd_train_step(params, xs, xt, labels, BETA, mu, cfg, 0.003, masks=m1, masks2=m2,
+    l32, _, _, gr32 = mcd.mcd_train_step(params, xs, xt, labels, beta, mu, cfg, 0.003, masks=m1, masks2=m2,
                                          gates=g1, gates2=gt2)
     assert_close(loss, l64, TOL[engine], f"{what} loss", noise=max(abs(l32.item() - l64.item()), 1e-7))
-    named = dict(step.model.named_parameters())
-    for name, go in gr64.items():
-        assert named[name].grad is not None, name
-        assert_close(named[name].grad, go, PINNED_TOL[engine], f"{what} grad {name}",
-                     noise=abs_err(gr32[name], go) * NOISE_SCALE[engine])
+    return assert_pinned_grads(dict(step.model.named_parameters()), gr64, gr32, engine, what, noise_floor)
 
 
 @gpu
