@@ -7,7 +7,8 @@
 //   warp 8      : TMA producer -- cp.async.bulk.tensor into a ring of 128B-swizzled stages (mbarrier handshake)
 //   warps 9..11 : B preparation -- write a K-major copy of each landed B tile beside it when B is MN-major (and, in
 //                 the precise kernel, the tf32 lo part of B), then arrive on the stage's ready barrier
-// setmaxnreg gives the producer warpgroup 40 registers per thread and the consumers 232.
+// setmaxnreg gives the producer warpgroup 40 registers per thread and the consumers 232 (64 / 216 in the plain kernel
+// with MN-major B, whose B warps keep two transpose blocks in flight).
 // Operands stay fp32 in HBM: the tf32 MMA reads the fp32 bit patterns (10-bit mantissa, fp32 range), so there is no
 // conversion pass and no second copy of any tensor in global memory.
 // The "gather" of TRN frame tuples, the source/target split and the per-frame dgrad are all
@@ -49,16 +50,32 @@ constexpr int TC_B_THREADS = 32 * TC_B_WARPS;
 constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;
 static_assert(128 * TC_PRODUCER_REGS + 256 * TC_CONSUMER_REGS <= TC_THREADS * 168,
               "setmaxnreg budget exceeds the registers of one CTA");
+// The plain kernel with MN-major B: the B warps keep two blocks of the transpose in flight (tc_transpose_b, 32
+// registers of data), and its consumers (64 accumulators, two slabs of A fragments) need fewer than the precise
+// kernel's, which hold 64 running sums and hi / lo fragments besides.
+constexpr int TC_XPOSE_PRODUCER_REGS = 64, TC_XPOSE_CONSUMER_REGS = 216;
+static_assert(128 * TC_XPOSE_PRODUCER_REGS + 256 * TC_XPOSE_CONSUMER_REGS <= TC_THREADS * 168,
+              "setmaxnreg budget exceeds the registers of one CTA");
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 4;   // 16 KB
 constexpr int TC_B_BYTES = TC_BN * TC_BK * 4;   // 16 KB
 constexpr int TC_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;
-// 4 stages (one CTA per SM; 129 KB of ring, or 193 KB when the plain kernel keeps a K-major copy of MN-major B, as the
-// precise kernel always does): the grids of this workload are within a wave, so a CTA is alone on its SM and bound by
-// TMA latency -- the bytes in flight per CTA matter more than a second resident CTA.
+// 4 stages (one CTA per SM; 129 KB of ring, or 193 KB when the precise kernel keeps its lo tile of B beside each
+// stage): the grids of this workload are within a wave, so a CTA is alone on its SM and bound by TMA latency -- the
+// bytes in flight per CTA matter more than a second resident CTA.
 constexpr int TC_STAGES = 4;
-// the plain kernel's stage: [A | B] as loaded, + [B K-major] when B is MN-major
-__host__ __device__ constexpr int tc_stage_bytes(bool b_kmaj) { return TC_STAGE_BYTES + (b_kmaj ? 0 : TC_B_BYTES); }
-constexpr int tc_smem_bytes(bool b_kmaj) { return TC_STAGES * tc_stage_bytes(b_kmaj) + 1024; }   // + alignment slack
+// With MN-major B the plain kernel keeps two rings: the raw stages [A | B as loaded] (32 KB) and the K-major copies of
+// B (16 KB).  A raw stage is free again once the consumers hold its A fragments in registers and the B warps have
+// transposed its B, long before the MMAs that read the copy retire: TMA runs up to TC_RAW_STAGES slabs ahead, the B
+// warps up to TC_KB_STAGES ahead of the MMAs.  5 x 32 + 3 x 16 = 208 KB (+ the slack and the ~4.3 KB of static
+// tables: 227 KB is the opt-in limit).
+constexpr int TC_RAW_STAGES = 5, TC_KB_STAGES = 3;
+constexpr int kTcMaxStages = 8;
+static_assert(TC_STAGES <= kTcMaxStages && TC_RAW_STAGES <= kTcMaxStages && TC_KB_STAGES <= kTcMaxStages,
+              "ring deeper than its barrier arrays");
+__host__ __device__ constexpr int tc_raw_stages(bool b_kmaj) { return b_kmaj ? TC_STAGES : TC_RAW_STAGES; }
+constexpr int tc_smem_bytes(bool b_kmaj) {       // + alignment slack
+  return tc_raw_stages(b_kmaj) * TC_STAGE_BYTES + (b_kmaj ? 0 : TC_KB_STAGES * TC_B_BYTES) + 1024;
+}
 #ifndef TA3N_MAX_MAPS
 #define TA3N_MAX_MAPS 64
 #endif
@@ -198,33 +215,60 @@ __device__ __forceinline__ float tf32_hi(float a) { return __uint_as_float(__flo
 __device__ __forceinline__ float f4_at(const float4& v, int i) { return i == 0 ? v.x : i == 1 ? v.y : i == 2 ? v.z : v.w; }
 
 // One 4 x 4 block (m = 4mq.., k = 4kq..) of an MN-major operand tile, block t of 256: read by tc_prep_load, written
-// K-major (transposed) by tc_prep_store; the block map keeps the 16 B stores of 32 consecutive blocks conflict-free
-// and the loads at most 2-way.
+// K-major (transposed) by tc_prep_store.  A 16 B access is served per quarter warp (8 consecutive blocks), so both
+// are conflict-free when those 8 blocks hit 8 different 16 B chunks of the 128 B bank row:
+//   load  chunk (mq & 7) ^ (k & 7), k = 4 kq + i:  bits (mq0, mq1, mq2 ^ kq0)
+//   store chunk  kq ^ (m & 7),      m = 4 mq + i:  bits (kq0, kq1, kq2 ^ mq0)
+// t0 -> mq0, t1 -> mq1 and kq1, t2 -> kq0 make both sets distinct over t0..t2; t7 gives kq1 its own bit
+// (kq1 = t1 ^ t7), so the map is a bijection of the 256 blocks.
 __device__ __forceinline__ void tc_prep_blk(const int t, int* mq, int* kq) {
-  *mq = (t & 1) | (((t >> 3) & 15) << 1);
-  *kq = ((t >> 1) & 3) | (((t >> 7) & 1) << 2);
+  *mq = (t & 3) | (((t >> 3) & 7) << 2);
+  *kq = ((t >> 2) & 1) | ((((t >> 1) ^ (t >> 7)) & 1) << 1) | (((t >> 6) & 1) << 2);
 }
+// Row i of block t sits at (tile + off) ^ (i << 4), + 128 i, in either tile: off keeps the SW128 chunk of row 0 in
+// bits 4..6 and bits 7..8 clear, and tiles are 1024-B aligned.  One offset per block and tile (not four) stays live.
+//   MN-major: mnmaj_chunk(4 kq + i, mq) = (mq >> 3) 4096 + 512 kq + 128 i + (((mq & 7) ^ 4 (kq & 1) ^ i) << 4)
+//   K-major:  kmaj_chunk(4 mq + i, kq)  = 512 mq + 128 i + ((kq ^ 4 (mq & 1) ^ i) << 4)
 __device__ __forceinline__ void tc_prep_load(const uint32_t base, const int t, float4 (&r)[4]) {
   int mq, kq;
   tc_prep_blk(t, &mq, &kq);
+  const uint32_t p = base + (uint32_t)((mq >> 3) * 4096 + 512 * kq + (((mq & 7) ^ (4 * (kq & 1))) << 4));
 #pragma unroll
-  for (int i = 0; i < 4; ++i) r[i] = lds4(base + mnmaj_chunk(4 * kq + i, mq));
+  for (int i = 0; i < 4; ++i) r[i] = lds4((p ^ (i << 4)) + 128u * i);
 }
 __device__ __forceinline__ void tc_prep_store(const uint32_t base, const int t, const float4 (&r)[4]) {
   int mq, kq;
   tc_prep_blk(t, &mq, &kq);
+  const uint32_t p = base + (uint32_t)(512 * mq + ((kq ^ (4 * (mq & 1))) << 4));
 #pragma unroll
   for (int i = 0; i < 4; ++i)
-    sts4(base + kmaj_chunk(4 * mq + i, kq), make_float4(f4_at(r[0], i), f4_at(r[1], i), f4_at(r[2], i), f4_at(r[3], i)));
+    sts4((p ^ (i << 4)) + 128u * i, make_float4(f4_at(r[0], i), f4_at(r[1], i), f4_at(r[2], i), f4_at(r[3], i)));
 }
 // B preparation warps (thread t of 96): the MN-major B tile at b_mn, transposed into the K-major SW128 tile at b_k.
+// Thread t moves blocks t, t + 96 and (t < 64) t + 192.  Under the MMAs' operand reads a shared-memory load takes
+// hundreds of cycles; with TWO_IN_FLIGHT the loads of two blocks are in flight together and the third block's are
+// issued before the second block is stored: two load round trips per tile instead of three, for 32 registers of data
+// (the plain kernel; the precise kernel's split warps have 40 registers and move one block at a time).
+static_assert(2 * TC_B_THREADS < 256 && 256 <= 3 * TC_B_THREADS, "tc_transpose_b moves two or three blocks per thread");
+template <bool TWO_IN_FLIGHT>
 __device__ __forceinline__ void tc_transpose_b(const uint32_t b_mn, const uint32_t b_k, const int t) {
+  if (!TWO_IN_FLIGHT) {
 #pragma unroll 1
-  for (int blk = t; blk < 256; blk += TC_B_THREADS) {
-    float4 r[4];
-    tc_prep_load(b_mn, blk, r);
-    tc_prep_store(b_k, blk, r);
+    for (int blk = t; blk < 256; blk += TC_B_THREADS) {
+      float4 r[4];
+      tc_prep_load(b_mn, blk, r);
+      tc_prep_store(b_k, blk, r);
+    }
+    return;
   }
+  const bool third = t + 2 * TC_B_THREADS < 256;
+  float4 r[4], q[4];
+  tc_prep_load(b_mn, t, r);
+  tc_prep_load(b_mn, t + TC_B_THREADS, q);
+  tc_prep_store(b_k, t, r);
+  if (third) tc_prep_load(b_mn, t + 2 * TC_B_THREADS, r);
+  tc_prep_store(b_k, t + TC_B_THREADS, q);
+  if (third) tc_prep_store(b_k, t + 2 * TC_B_THREADS, r);
 }
 
 // Per-thread part of the A fragment addresses of rows m = r0 (and r0 + 8, MN-major), column k = tq: the word offset
@@ -254,20 +298,63 @@ __device__ __forceinline__ void tc_load_a(const uint32_t a_base, const uint32_t 
     }
 }
 
+#ifdef TA3N_TC_TIMELINE
+// Stage timeline of the plain kernel (tools/tc_stage_timeline.py; off in the product build): clock64 stamps of the
+// first kTlSlabs slabs of every CTA, by event, and each CTA's globaltimer and clock64 at its start and end (the SM
+// clock while it ran).  The producer stamps TMA issue; B warp 9 lane 0 the landed stage and the transpose; consumer
+// thread 0 the rest.
+constexpr int kTlCtas = 132, kTlSlabs = 64, kTlEvents = 9;
+enum : int {
+  TL_TMA_ISSUE,      // producer: the stage is free, TMA issued
+  TL_FULL,           // B warps: the raw stage has landed
+  TL_XPOSE_START,    // B warps: K-major slot free, transpose starts
+  TL_XPOSE_END,      // B warps: transposed and fenced, ready arrived
+  TL_CONS_START,     // consumers: slab entered
+  TL_READY,          // consumers: A landed and B ready
+  TL_RELEASED,       // consumers: MMAs issued, raw stage (MN-major B) released
+  TL_RETIRED,        // consumers: the slab's MMAs retired
+  TL_FENCE,          // B warps: transpose stores issued, proxy fence next
+};
+__device__ unsigned long long g_tc_tl[kTlCtas][kTlSlabs][kTlEvents];
+__device__ unsigned long long g_tc_tl_clk[kTlCtas][4];   // globaltimer, clock64 at start; globaltimer, clock64 at end
+__device__ __forceinline__ unsigned long long tl_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ void tl_stamp(const uint32_t slab, const int ev) {
+  if (blockIdx.x < kTlCtas && slab < (uint32_t)kTlSlabs) g_tc_tl[blockIdx.x][slab][ev] = clock64();
+}
+__device__ __forceinline__ void tl_clock(const int at_end) {
+  if (blockIdx.x < kTlCtas) {
+    g_tc_tl_clk[blockIdx.x][2 * at_end] = tl_globaltimer();
+    g_tc_tl_clk[blockIdx.x][2 * at_end + 1] = clock64();
+  }
+}
+#define TA3N_TL(cond, slab, ev) \
+  do {                          \
+    if (cond) tl_stamp((uint32_t)(slab), (ev)); \
+  } while (0)
+#else
+#define TA3N_TL(cond, slab, ev) ((void)0)
+#endif
+
 // ---- one output tile, by warp role ---------------------------------------------------------------------
 // The operand ring barriers are initialised once per CTA.  The precise kernel's producer runs ahead over its task
 // list (it fills the ring with the slabs of task t+1 while the consumer warps still finish task t), so it passes its
 // running slab count to tc_produce.
 struct TcShared {
-  uint64_t full_bar[4];      // TMA landed
-  uint64_t empty_bar[4];     // every consumer warp is done with the stage
+  uint64_t full_bar[kTcMaxStages];      // TMA landed
+  uint64_t empty_bar[kTcMaxStages];     // every reader of the stage is done with it
 };
 
+// `readers`: warps that arrive on a stage's empty barrier (the consumer warps, + the B warps when they read the raw
+// stage and the consumers release it before their MMAs retire)
 template <int STAGES>
-__device__ __forceinline__ void tc_pipe_init(TcShared* sh) {
+__device__ __forceinline__ void tc_pipe_init(TcShared* sh, const int readers = TC_CONSUMER_WARPS) {
   for (int s = 0; s < STAGES; ++s) {
     mbar_init(&sh->full_bar[s], 1);
-    mbar_init(&sh->empty_bar[s], TC_CONSUMER_WARPS);
+    mbar_init(&sh->empty_bar[s], readers);
   }
   fence_barrier_init();
 }
@@ -298,6 +385,7 @@ __device__ __forceinline__ void tc_produce(const TileCtx& ctx, const CUtensorMap
     const int stage = (int)(gl % STAGES);
     const uint32_t phase = (gl / STAGES) & 1u;
     mbar_wait(&sh->empty_bar[stage], phase ^ 1u);
+    TA3N_TL(true, gl, TL_TMA_ISSUE);
     mbar_expect_tx(&sh->full_bar[stage], TC_STAGE_BYTES);
     uint8_t* sA = smem + stage * STAGE_BYTES;
     uint8_t* sB = sA + TC_A_BYTES;
@@ -453,24 +541,36 @@ __device__ __forceinline__ void frag_finish(const Group& g, const int split, con
 }
 
 // ---- the plain kernel ("tf32"): one tile per CTA ---------------------------------------------------------------
-// Warp 8 lane 0 issues the TMA loads; for MN-major B, warps 9..11 write the K-major copy of each landed B tile beside
-// it and mark the stage ready.  The consumers load their A fragments from the landed A tile (either layout) and issue
-// one product per K step with B from shared memory: they do nothing else in the K loop.  Per slab and CTA, shared
-// memory moves 32 KB of TMA fill, 16 KB of A fragment loads and 32 KB of B operand reads (each warpgroup reads all of
-// B), + 32 KB for the transpose of MN-major B.
+// Warp 8 lane 0 issues the TMA loads; for MN-major B, warps 9..11 write the K-major copy of each landed B tile into
+// a ring of its own (TC_KB_STAGES) and mark it ready.  The consumers load their A fragments from the landed A tile
+// (either layout) and issue one product per K step with B from shared memory: they do nothing else in the K loop.
+// Per slab and CTA, shared memory moves 32 KB of TMA fill, 16 KB of A fragment loads and 32 KB of B operand reads
+// (each warpgroup reads all of B), + 32 KB for the transpose of MN-major B.
+//
+// Ring hand-offs.  K-major B: one ring of TC_STAGES [A | B] stages, released by the consumers once the stage's MMAs
+// have retired.  MN-major B: the raw stage (full_bar / empty_bar, TC_RAW_STAGES) is released by the 8 consumer warps
+// once its A fragments are in registers (after the MMAs that read them are issued) and by the 3 B warps after its
+// transpose; the K-major copy (kready_bar / kempty_bar, TC_KB_STAGES) is released by the consumers once the MMAs
+// that read it have retired.
 
 // Consumer warpgroups: slab `it` of the tile, A fragments in `a` (not the set of the group still in flight).  Leaves
-// this slab's group in flight and releases the previous stage.
+// this slab's group in flight and releases what the previous slab's MMAs read: its stage (K-major B) or its K-major
+// copy of B (MN-major B; the raw stage of this slab is released as soon as its MMAs are issued).
 template <bool A_KMAJ, bool B_KMAJ>
-__device__ __forceinline__ void tc_consume_slab(const uint32_t it, uint8_t* smem, TcShared* sh, uint64_t* ready_bar,
-                                                const uint32_t off0, const uint32_t off1, uint32_t (&a)[16],
-                                                float (&d)[64], int& prev) {
-  const int stage = (int)(it % TC_STAGES);
-  const uint32_t parity = (it / TC_STAGES) & 1u;
+__device__ __forceinline__ void tc_consume_slab(const uint32_t it, uint8_t* smem, TcShared* sh, uint64_t* kready_bar,
+                                                uint64_t* kempty_bar, const uint32_t off0, const uint32_t off1,
+                                                uint32_t (&a)[16], float (&d)[64], int& prev) {
+  constexpr int kRaw = tc_raw_stages(B_KMAJ);
+  const int stage = (int)(it % kRaw);
+  const uint32_t parity = (it / kRaw) & 1u;
+  const int kst = (int)(it % TC_KB_STAGES);
+  TA3N_TL(threadIdx.x == 0, it, TL_CONS_START);
   mbar_wait(&sh->full_bar[stage], parity);          // A landed (read below with ordinary loads)
-  if (!B_KMAJ) mbar_wait(&ready_bar[stage], parity);  // K-major copy of B written
-  const uint32_t a_base = smem_u32(smem + stage * tc_stage_bytes(B_KMAJ));
-  const uint32_t b_base = a_base + TC_A_BYTES + (B_KMAJ ? 0 : TC_B_BYTES);
+  if (!B_KMAJ) mbar_wait(&kready_bar[kst], (it / TC_KB_STAGES) & 1u);   // K-major copy of B written
+  TA3N_TL(threadIdx.x == 0, it, TL_READY);
+  const uint32_t a_base = smem_u32(smem + stage * TC_STAGE_BYTES);
+  const uint32_t b_base = B_KMAJ ? a_base + TC_A_BYTES
+                                 : smem_u32(smem + TC_RAW_STAGES * TC_STAGE_BYTES + kst * TC_B_BYTES);
   tc_load_a<A_KMAJ>(a_base, off0, off1, a);
 #pragma unroll
   for (int j = 0; j < 16; ++j) reg_fence(a[j]);
@@ -481,24 +581,34 @@ __device__ __forceinline__ void tc_consume_slab(const uint32_t it, uint8_t* smem
     wgmma_tf32_rs(d, a[f], a[f + 1], a[f + 2], a[f + 3], wgmma_desc(b_base, ks));
   }
   wgmma_commit();
-  wgmma_wait<1>();                                  // the previous slab's MMAs are done: release its stage
-  if (prev >= 0) {
+  if (!B_KMAJ) {                                    // the MMAs took the A registers: the raw stage is read
     __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(&sh->empty_bar[prev]);
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&sh->empty_bar[stage]);
+    TA3N_TL(threadIdx.x == 0, it, TL_RELEASED);
   }
-  prev = stage;
+  wgmma_wait<1>();                                  // the previous slab's MMAs are done: release what they read
+  if (prev >= 0) {
+    TA3N_TL(threadIdx.x == 0, it - 1, TL_RETIRED);
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(B_KMAJ ? &sh->empty_bar[prev] : &kempty_bar[prev]);
+  }
+  prev = B_KMAJ ? stage : kst;
 }
 
 template <bool A_KMAJ, bool B_KMAJ>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 seg_gemm_tc_kernel(const __grid_constant__ GemmTable tab, const __grid_constant__ TcMaps maps,
                    const __grid_constant__ TcSegMaps segmaps, const int first_wave) {
-  constexpr int kStageBytes = tc_stage_bytes(B_KMAJ);
+  constexpr int kRaw = tc_raw_stages(B_KMAJ);
   extern __shared__ uint8_t tc_smem_raw[];
   __shared__ __align__(8) TcShared sh;
-  __shared__ __align__(8) uint64_t ready_bar[TC_STAGES];     // B transposed (one arrival per B warp)
+  __shared__ __align__(8) uint64_t kready_bar[TC_KB_STAGES];    // B transposed (one arrival per B warp)
+  __shared__ __align__(8) uint64_t kempty_bar[TC_KB_STAGES];    // the MMAs that read the copy retired (consumer warps)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#ifdef TA3N_TC_TIMELINE
+  if (threadIdx.x == 0) tl_clock(0);
+#endif
 
   // ---- tile decode (same scheme as the SIMT engine, 128x128 tiles); group + segments staged in smem ----
   __shared__ TileCtx ctx;
@@ -512,8 +622,11 @@ seg_gemm_tc_kernel(const __grid_constant__ GemmTable tab, const __grid_constant_
   tc_chunk_range(ctx, split, &c_begin, &n_iter);
 
   if (warp == TC_CONSUMER_WARPS && lane == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) mbar_init(&ready_bar[s], TC_B_WARPS);
-    tc_pipe_init<TC_STAGES>(&sh);
+    for (int s = 0; s < TC_KB_STAGES; ++s) {
+      mbar_init(&kready_bar[s], TC_B_WARPS);
+      mbar_init(&kempty_bar[s], TC_CONSUMER_WARPS);
+    }
+    tc_pipe_init<kRaw>(&sh, TC_CONSUMER_WARPS + (B_KMAJ ? 0 : TC_B_WARPS));
   }
   __syncthreads();
   // Everything above touched only kernel parameters and shared memory: it overlaps the previous kernel of the
@@ -521,47 +634,59 @@ seg_gemm_tc_kernel(const __grid_constant__ GemmTable tab, const __grid_constant_
   pdl_wait();
 
   if (warp >= TC_CONSUMER_WARPS) {
-    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    setmaxnreg_dec<B_KMAJ ? TC_PRODUCER_REGS : TC_XPOSE_PRODUCER_REGS>();
     if (warp == TC_CONSUMER_WARPS) {
       if (lane == 0 && n_iter > 0)
-        tc_produce<TC_STAGES, kStageBytes>(ctx, maps.m, A_KMAJ, B_KMAJ, tab.pad_, m0, n0, c_begin, n_iter, smem, &sh,
-                                           0u);
+        tc_produce<kRaw, TC_STAGE_BYTES>(ctx, maps.m, A_KMAJ, B_KMAJ, tab.pad_, m0, n0, c_begin, n_iter, smem, &sh, 0u);
     } else if (!B_KMAJ) {
       const int t = threadIdx.x - 32 * (TC_CONSUMER_WARPS + 1);
+      const uint32_t kring = smem_u32(smem + TC_RAW_STAGES * TC_STAGE_BYTES);
       for (int it = 0; it < n_iter; ++it) {
-        const int stage = it % TC_STAGES;
-        mbar_wait(&sh.full_bar[stage], (uint32_t)(it / TC_STAGES) & 1u);
-        const uint32_t b_mn = smem_u32(smem + stage * kStageBytes) + TC_A_BYTES;
-        tc_transpose_b(b_mn, b_mn + TC_B_BYTES, t);
+        const int stage = it % TC_RAW_STAGES, kst = it % TC_KB_STAGES;
+        mbar_wait(&sh.full_bar[stage], (uint32_t)(it / TC_RAW_STAGES) & 1u);
+        TA3N_TL(t == 0, it, TL_FULL);
+        mbar_wait(&kempty_bar[kst], ((uint32_t)(it / TC_KB_STAGES) & 1u) ^ 1u);
+        TA3N_TL(t == 0, it, TL_XPOSE_START);
+        tc_transpose_b<true>(smem_u32(smem + stage * TC_STAGE_BYTES) + TC_A_BYTES, kring + kst * TC_B_BYTES, t);
+        TA3N_TL(t == 0, it, TL_FENCE);
         fence_proxy_async();            // generic-proxy writes -> the tensor core's reads
         __syncwarp();
-        if (lane == 0) mbar_arrive(&ready_bar[stage]);
+        if (lane == 0) {
+          mbar_arrive(&kready_bar[kst]);
+          mbar_arrive(&sh.empty_bar[stage]);
+        }
+        TA3N_TL(t == 0, it, TL_XPOSE_END);
       }
     }
   } else {
-    setmaxnreg_inc<TC_CONSUMER_REGS>();
+    setmaxnreg_inc<B_KMAJ ? TC_CONSUMER_REGS : TC_XPOSE_CONSUMER_REGS>();
     const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);      // fragment rows r0, r0 + 8
     const uint32_t off0 = tc_a_thread_off<A_KMAJ>(r0, lane & 3), off1 = tc_a_thread_off<A_KMAJ>(r0 + 8, lane & 3);
     float d[64];
 #pragma unroll
     for (int j = 0; j < 64; ++j) d[j] = 0.f;
     uint32_t a[2][16];                  // A fragments of the even / odd slabs
-    int prev = -1;                      // stage whose MMAs may still be in flight
+    int prev = -1;                      // stage (or K-major slot) whose MMAs may still be in flight
     // The odd last slab is peeled off the loop: with the pair's second slab conditional inside it, the back edge would
     // let one register set be rewritten while its own group is in flight, and ptxas would serialize every MMA (C7513).
     int it = 0;
     for (; it + 1 < n_iter; it += 2) {
-      tc_consume_slab<A_KMAJ, B_KMAJ>((uint32_t)it, smem, &sh, ready_bar, off0, off1, a[0], d, prev);
-      tc_consume_slab<A_KMAJ, B_KMAJ>((uint32_t)(it + 1), smem, &sh, ready_bar, off0, off1, a[1], d, prev);
+      tc_consume_slab<A_KMAJ, B_KMAJ>((uint32_t)it, smem, &sh, kready_bar, kempty_bar, off0, off1, a[0], d, prev);
+      tc_consume_slab<A_KMAJ, B_KMAJ>((uint32_t)(it + 1), smem, &sh, kready_bar, kempty_bar, off0, off1, a[1], d, prev);
     }
-    if (it < n_iter) tc_consume_slab<A_KMAJ, B_KMAJ>((uint32_t)it, smem, &sh, ready_bar, off0, off1, a[0], d, prev);
+    if (it < n_iter)
+      tc_consume_slab<A_KMAJ, B_KMAJ>((uint32_t)it, smem, &sh, kready_bar, kempty_bar, off0, off1, a[0], d, prev);
     wgmma_wait<0>();
     if (prev >= 0) {
+      TA3N_TL(threadIdx.x == 0, n_iter - 1, TL_RETIRED);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&sh.empty_bar[prev]);
+      if (lane == 0) mbar_arrive(B_KMAJ ? &sh.empty_bar[prev] : &kempty_bar[prev]);
     }
     frag_finish(ctx.g, split, m0, n0, d);
   }
+#ifdef TA3N_TC_TIMELINE
+  if (threadIdx.x == 0) tl_clock(1);
+#endif
 }
 
 // ---- the precise forward kernel ("tf32x3"): fp32-grade products from the tensor cores -------------------------
@@ -658,7 +783,7 @@ template <bool B_KMAJ>
 __device__ __forceinline__ void x3_split_b(const uint32_t b_raw, const uint32_t b_lo, const int t) {
   uint32_t src = b_raw;
   if (!B_KMAJ) {
-    tc_transpose_b(b_raw, b_lo, t);
+    tc_transpose_b<false>(b_raw, b_lo, t);
     x3_split_sync();                  // every read of the raw tile before the K-major writes over it
     src = b_lo;
   }

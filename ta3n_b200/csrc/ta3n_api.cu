@@ -1483,4 +1483,18 @@ int ta3n_gemm_ex(const float* A, int lda, int a_kmajor, const float* B, int ldb,
   return run_gemm(plan, S(stream), workspace ? &arena : nullptr);
 }
 
+#ifdef TA3N_TC_TIMELINE
+// Instrumented builds only (tools/tc_stage_timeline.py): copy the plain kernel's stage timeline to `host`
+// (g_tc_tl, then g_tc_tl_clk) and clear it for the next launch.
+int ta3n_tc_timeline_read(void* host, size_t bytes) {
+  TA3N_REQUIRE(host && bytes == sizeof(g_tc_tl) + sizeof(g_tc_tl_clk), "bad arguments");
+  TA3N_CUDA(cudaDeviceSynchronize());
+  TA3N_CUDA(cudaMemcpyFromSymbol(host, g_tc_tl, sizeof(g_tc_tl)));
+  TA3N_CUDA(cudaMemcpyFromSymbol(static_cast<char*>(host) + sizeof(g_tc_tl), g_tc_tl_clk, sizeof(g_tc_tl_clk)));
+  static const unsigned long long zero[kTlCtas][kTlSlabs][kTlEvents] = {};
+  TA3N_CUDA(cudaMemcpyToSymbol(g_tc_tl, zero, sizeof(g_tc_tl)));
+  return TA3N_OK;
+}
+#endif
+
 }  // extern "C"
