@@ -285,6 +285,14 @@ int ta3n_ce_loss_fwd_bwd(const float* pred, const long long* labels, int rows, i
  * so that the buffer it lives in can carry the other pass's gradient.                                            */
 int ta3n_mcd_loss_fwd_bwd(const float* pred1, const float* pred2, int rows, int C, const int* valid_rows, float* loss,
                           float* g_pred1, float* g_pred2, float* g_move1, ta3n_stream_t stream);
+/* ---- entropy of the target predictions, add_loss_DA 'target_entropy' (main.py:541-545; loss.py:8-12) ----------- */
+/* One single-block launch, rows summed in fp64 in a fixed order (replays are bit-identical).  On the real rows
+ * r < valid_rows[1] (valid_rows: the {real source rows, real target rows} pair of ta3n_loss_fwd_bwd; NULL = rows):
+ *   term = mean_r H(softmax(pred[r])),  loss += gamma * term,  g_pred [rows,C] += the gradient of gamma * term.
+ * Padded rows of g_pred are left untouched; no real row (or rows == 0) adds nothing.  meter (optional, 3 doubles):
+ * {sum += term * n, last = term, count += n}, n = the real rows (the losses_e meter of main.py:544).              */
+int ta3n_target_entropy_fwd_bwd(const float* pred, int rows, int C, float gamma, const int* valid_rows, float* loss,
+                                float* g_pred, double* meter, ta3n_stream_t stream);
 /* dst[i] += src[i] for n floats (both 16-byte aligned): sums the gradient buckets of two backward passes.          */
 int ta3n_accumulate(float* dst, const float* src, long long n, ta3n_stream_t stream);
 

@@ -106,6 +106,7 @@ SIGNATURES = {
     "ta3n_counter_inc": (_I, [_VP, _VP]),
     "ta3n_ce_loss_fwd_bwd": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP]),
     "ta3n_mcd_loss_fwd_bwd": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "ta3n_target_entropy_fwd_bwd": (_I, [_VP, _I, _I, _F, _VP, _VP, _VP, _VP, _VP]),
     "ta3n_accumulate": (_I, [_VP, _VP, C.c_longlong, _VP]),
     "ta3n_discrepancy_workspace_bytes": (_SZ, [_I, _I, _I]),
     "ta3n_discrepancy_fwd_bwd": (_I, [_I, _I, _I, _VP, _VP, _I, _I, _F, _VP, _VP, _VP, _VP, _I, _I, _F, _VP, _VP,

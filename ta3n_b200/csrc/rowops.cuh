@@ -839,6 +839,59 @@ mcd_loss_kernel(const float* __restrict__ p1, const float* __restrict__ p2, int 
   block_add_scalar(acc, -inv, loss);
 }
 
+constexpr int kEntThreads = 1024;
+
+// Entropy of the target predictions, --add_loss_DA target_entropy (main.py:541-545, loss.py:8-12), on the real rows
+// r < valid_rows[1]:
+//   term = 1/n sum_r H_r,  H_r = -sum_c q_rc log q_rc,  q = softmax over C;  loss += gamma * term
+//   g_pred[r] += gamma/n * (-q_rc (log q_rc + H_r))   (padded rows untouched)
+// Warp w of 32 takes rows w, w + 32, ... (a row costs a few dependent warp reductions, so the block is as wide as it
+// gets); the row entropies are summed in fp64, per warp in row order and then the warps in order, so the term is the
+// same bit pattern on every replay.  n == 0 adds nothing.
+// meter (optional, 3 doubles): {sum += term * n, last = term, count += n} -- the losses_e meter of main.py:544.
+__global__ void __launch_bounds__(kEntThreads)
+target_entropy_kernel(const float* __restrict__ pred, int rows, int C, float gamma, const int* __restrict__ valid_rows,
+                      float* __restrict__ loss, float* __restrict__ g_pred, double* __restrict__ meter) {
+  pdl_wait();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int vt = valid_rows ? max(0, min(valid_rows[1], rows)) : rows;
+  const float scale = gamma / (float)max(vt, 1);
+  double acc = 0.0;   // lane 0: this warp's sum of H_r
+  for (int r = warp; r < vt; r += kEntThreads / 32) {
+    const float* p = pred + (size_t)r * C;
+    float* g = g_pred + (size_t)r * C;
+    const float mx = row_max(p, C, lane);
+    float se = 0.f;
+    for (int c = lane; c < C; c += 32) se += expf(p[c] - mx);
+    const float lse = logf(warp_sum(se));
+    float h = 0.f;
+    for (int c = lane; c < C; c += 32) {
+      const float lq = p[c] - mx - lse;
+      h -= expf(lq) * lq;
+    }
+    h = warp_sum(h);
+    for (int c = lane; c < C; c += 32) {
+      const float lq = p[c] - mx - lse;
+      g[c] += scale * (-expf(lq) * (lq + h));
+    }
+    if (lane == 0) acc += (double)h;
+  }
+  __shared__ double red[kEntThreads / 32];
+  if (lane == 0) red[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int w = 0; w < kEntThreads / 32; ++w) t += red[w];
+    const double term = vt > 0 ? t / (double)vt : 0.0;
+    if (vt > 0) loss[0] += (float)((double)gamma * term);
+    if (meter) {
+      meter[0] += term * (double)vt;
+      meter[1] = term;
+      meter[2] += (double)vt;
+    }
+  }
+}
+
 // dst += src (n floats)
 __global__ void __launch_bounds__(256) accumulate_kernel(float* __restrict__ dst, const float* __restrict__ src,
                                                          size_t n) {

@@ -1039,6 +1039,18 @@ int ta3n_mcd_loss_fwd_bwd(const float* pred1, const float* pred2, int rows, int 
   return after_launch();
 }
 
+int ta3n_target_entropy_fwd_bwd(const float* pred, int rows, int C, float gamma, const int* valid_rows, float* loss,
+                                float* g_pred, double* meter, ta3n_stream_t stream) {
+  TA3N_REQUIRE(rows >= 0 && C >= 1, "bad sizes");
+  if (rows == 0) return TA3N_OK;
+  TA3N_REQUIRE(pred && loss && g_pred, "null pointer");
+  TA3N_REQUIRE((const float*)g_pred != pred && (const float*)loss != pred, "outputs must not alias pred");
+  pre_launch("target_entropy", S(stream));
+  launch_kernel(target_entropy_kernel, 1, kEntThreads, 0, S(stream), pred, rows, C, gamma, valid_rows, loss, g_pred,
+                meter);
+  return after_launch();
+}
+
 int ta3n_accumulate(float* dst, const float* src, long long n, ta3n_stream_t stream) {
   TA3N_REQUIRE(n >= 0, "bad size");
   if (n == 0) return TA3N_OK;

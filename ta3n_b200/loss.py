@@ -29,7 +29,8 @@ def dis_MCD(out1, out2):
 def ta3n_loss(outputs, label_source, gamma=0.003, place_adv=('Y', 'Y', 'Y'), use_attn='TransAttn',
               add_loss_DA='attentive_entropy'):
     """Loss of the shipped configuration (use_target='uSv', adv_DA='RevGrad'):
-    main.py:446 (source CE) + main.py:508-538 (domain CE per level) + main.py:559-562."""
+    main.py:446 (source CE) + main.py:508-538 (domain CE per level) + main.py:541-545 (target entropy; 0 without a
+    target row) or main.py:559-562 (attentive entropy)."""
     (_, out_s, _, pd_s, _, _, out_t, _, pd_t, _) = outputs
     loss = F.cross_entropy(out_s, label_source)
     per_level = []
@@ -42,6 +43,8 @@ def ta3n_loss(outputs, label_source, gamma=0.003, place_adv=('Y', 'Y', 'Y'), use
         both = torch.cat([ps, pt], 0)
         per_level.append(both)
         loss = loss + F.cross_entropy(both, dom)
+    if add_loss_DA == 'target_entropy' and out_t.size(0) > 0:
+        loss = loss + gamma * cross_entropy_soft(out_t)
     if add_loss_DA == 'attentive_entropy' and use_attn != 'none' and len(per_level) > 1:
         loss = loss + gamma * attentive_entropy(torch.cat([out_s, out_t], 0), per_level[1])
     return loss

@@ -140,8 +140,9 @@ def parse_train_stats(words, topk: Sequence[int]) -> TrainStats:
 class TrainStatsSnapshot:
     """``TrainStep.stats_async()``: the accumulator copied to pinned host memory behind an event."""
 
-    def __init__(self, host: torch.Tensor, event, topk: Tuple[int, ...], dis_host: Optional[torch.Tensor] = None):
-        self._host, self._event, self._topk, self._dis_host = host, event, topk, dis_host
+    def __init__(self, host: torch.Tensor, event, topk: Tuple[int, ...], dis_host: Optional[torch.Tensor] = None,
+                 ent_host: Optional[torch.Tensor] = None):
+        self._host, self._event, self._topk, self._dis_host, self._ent_host = host, event, topk, dis_host, ent_host
 
     def done(self) -> bool:
         return self._event.query()
@@ -152,11 +153,14 @@ class TrainStatsSnapshot:
         st = parse_train_stats(self._host.numpy(), self._topk)
         if self._dis_host is not None:
             st.loss_d = dis_meter(self._dis_host.numpy())
+        if self._ent_host is not None:
+            st.loss_e = dis_meter(self._ent_host.numpy())
         return st
 
 
 def dis_meter(words) -> Meter:
-    """The ``loss_d`` meter from its accumulator {sum of val * n, last val, sum of n} (3 doubles)."""
+    """A meter kept by its own loss launch -- ``loss_d``, or ``loss_e`` of the target entropy -- from its accumulator
+    {sum of val * n, last val, sum of n} (3 doubles)."""
     s, val, n = (float(x) for x in words)
     return Meter(val=val, avg=s / n if n else 0.0, sum=s, count=int(n))
 
@@ -441,7 +445,15 @@ class TrainStep:
         contributes 0 to the loss and the gradient (the reference fails on both).  Under MCD the term reads pass 1's
         outputs.  alpha: a device scalar, rescheduled by ``set_alpha`` (``alpha_dann`` per epoch) without re-capture;
         a negative alpha raises ValueError (main.py:231 reads it as "use the schedule", not as a weight).
-        With stats=True the ``loss`` meter includes alpha * loss_d and ``TrainStats.loss_d`` holds the term."""
+        With stats=True the ``loss`` meter includes alpha * loss_d and ``TrainStats.loss_d`` holds the term.
+
+        add_loss_DA: 'attentive_entropy' (main.py:559-562; needs use_attn and place_adv[0] == place_adv[1] == 'Y' to
+        act), 'target_entropy' or 'none'; any other value raises ValueError.  'target_entropy' (mode 'legacy'; class /
+        domain weights and a negative beta are refused) adds gamma * the mean entropy of softmax over the real target
+        rows' class logits (main.py:541-545, loss.py:8-12), one launch after the loss launches
+        (``ta3n_target_entropy_fwd_bwd``); a batch with no real target row contributes 0.  Under MCD it reads pass 1's
+        target logits (main.py:542 runs before the reverse pass).  With stats=True the ``loss`` meter includes gamma *
+        the term and ``TrainStats.loss_e`` holds the term, n = the real target rows (main.py:544)."""
         if optimizer is not None and not isinstance(optimizer, (SGDNesterov, Adam)):
             raise TypeError(f"optimizer must be SGDNesterov or Adam, got {type(optimizer).__name__}")
         if isinstance(optimizer, Adam):
@@ -494,6 +506,18 @@ class TrainStep:
                     tuple(float(w) for w in domain_weight) != (1.0, 1.0):
                 raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
                                           "(mode='phased'), which does not cover ens_DA='MCD'")
+            mode = "legacy"
+        if add_loss_DA not in ("none", "attentive_entropy", "target_entropy"):
+            raise ValueError(f"add_loss_DA must be 'none', 'attentive_entropy' or 'target_entropy', got {add_loss_DA!r}")
+        self.target_entropy = add_loss_DA == "target_entropy"
+        if self.target_entropy:
+            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
+                raise NotImplementedError("add_loss_DA='target_entropy' runs in mode='legacy' only (the step program "
+                                          "has no target-entropy term)")
+            if class_weight is not None or any(float(b) < 0 for b in beta) or \
+                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
+                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
+                                          "(mode='phased'), which does not cover add_loss_DA='target_entropy'")
             mode = "legacy"
         if dis_DA != "none":
             self._check_dis(dis_DA, alpha, mode, class_weight, beta, domain_weight, process_group, place_dis,
@@ -661,6 +685,10 @@ class TrainStep:
             self._init_mcd(seed, di, dv, offs)
         self._init_stats(stats, stats_topk)
         self._init_dis(dis_DA, alpha, place_dis)
+        if self.target_entropy and self.mcd and self.pred_video_t1 is None:
+            self.pred_video_t1 = torch.zeros(self.Bt, self.C, **f32)
+        self.ent_meter = torch.zeros(3, device=dev, dtype=torch.float64) \
+            if (self.target_entropy and self.keep_stats) else None
         self.outputs = None
         self.branch_stream = torch.cuda.Stream(device=dev) if parallel_branches else None
         self.overlap_wgrad = bool(overlap_wgrad)
@@ -716,6 +744,7 @@ class TrainStep:
         """Buffers of the discrepancy loss: alpha, the unscaled term, the video feature's gradient, the workspace and
         (stats) the loss_d meter; under MCD a copy of pass 1's target logits, which pass 2 overwrites."""
         self.dis_DA = dis_DA
+        self.pred_video_t1 = None
         if dis_DA == "none":
             return
         f32 = dict(device=self.device, dtype=torch.float32)
@@ -802,6 +831,8 @@ class TrainStep:
         st = parse_train_stats(self.stats_acc.cpu().numpy(), self.stats_topk)
         if self.dis_DA != "none":
             st.loss_d = dis_meter(self.dis_meter.cpu().numpy())
+        if self.ent_meter is not None:
+            st.loss_e = dis_meter(self.ent_meter.cpu().numpy())
         return st
 
     def stats_async(self) -> TrainStatsSnapshot:
@@ -814,9 +845,13 @@ class TrainStep:
         if self.dis_DA != "none":
             dis_host = torch.empty(3, dtype=torch.float64, pin_memory=True)
             dis_host.copy_(self.dis_meter, non_blocking=True)
+        ent_host = None
+        if self.ent_meter is not None:
+            ent_host = torch.empty(3, dtype=torch.float64, pin_memory=True)
+            ent_host.copy_(self.ent_meter, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
-        return TrainStatsSnapshot(host, ev, self.stats_topk, dis_host)
+        return TrainStatsSnapshot(host, ev, self.stats_topk, dis_host, ent_host)
 
     def reset_stats(self) -> None:
         """Start an epoch of meters (main.py builds fresh AverageMeters in every train() call): zeroes the accumulator
@@ -825,6 +860,8 @@ class TrainStep:
         self.stats_acc.zero_()
         if self.dis_DA != "none":
             self.dis_meter.zero_()
+        if self.ent_meter is not None:
+            self.ent_meter.zero_()
 
     def _stack_drops(self, seed, di):
         """dropout_i of the stacked shared layers: one seed per layer (``stack_seed``), the step counter as key."""
@@ -1154,7 +1191,7 @@ class TrainStep:
             w2, b2 = self.params[-2], self.params[-1]
             check(lib.ta3n_video_head_fwd(_P(saved["dropped"]), self.Bs, w2.shape[1], self.C, _P(w2), _P(b2), None,
                                           _P(self.head2_scratch), _P(self.pred2_s), st))
-            if self.dis_DA != "none" and self.pred_video_t1 is not None:
+            if self.pred_video_t1 is not None:
                 self.pred_video_t1.copy_(pred_video[self.Bs:])      # pass 2 writes its target logits over these
             saved2, dims2 = self._enqueue_mcd_pass2_forward(lib, st)
         check(lib.ta3n_loss_fwd_bwd(_P(pred_video), _P(self.labels), _P(pred_rel), _P(pred_dom), _P(pred_frame),
@@ -1168,6 +1205,12 @@ class TrainStep:
             check(lib.ta3n_mcd_loss_fwd_bwd(_P(pred_video[self.Bs:]), _P(self.pred2_t), self.Bt, self.C, _P(self.valid),
                                             _P(self.loss), _P(self.g_video_t), _P(self.g_video2_t),
                                             _P(self.g_video[self.Bs:]), st))
+        if self.target_entropy:
+            # main.py:541-545 reads pass 1's target logits (it runs before MCD's reverse pass); under MCD its gradient
+            # goes in after ta3n_mcd_loss_fwd_bwd has moved the target rows of g_video over to pass 2
+            pt = self.pred_video_t1 if self.mcd else pred_video[self.Bs:]
+            check(lib.ta3n_target_entropy_fwd_bwd(_P(pt), self.Bt, self.C, self.gamma, _P(self.valid), _P(self.loss),
+                                                  _P(self.g_video[self.Bs:]), _P(self.ent_meter), st))
         if self.dis_DA != "none":
             self._enqueue_dis(st, outputs[4], pred_video)
         if self.keep_stats:
