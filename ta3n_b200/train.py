@@ -41,6 +41,7 @@ _N_LATE = 6     # path_parameters()[0:6] = shared layer W,b + frame discriminato
 _ALIGN = 64     # floats: every tensor of a flat buffer starts 256-byte aligned (vector stores, TMA operands)
 _PASS2_KEY = 0x6A09E667F3BCC908     # seed of MCD's second pass = step seed ^ this (its masks differ from pass 1's)
 _STACK_KEY = 0xBB67AE8584CAA73B     # dropout seed of stacked shared layer l (add_fc > 1) = pass seed ^ (l - 1) * this
+_PRETRAIN_KEY = 0x3C6EF372FE94F82B  # seed of the source-only pre-training pass = step seed ^ this
 
 
 def stack_seed(seed: int, layer: int) -> int:
@@ -272,14 +273,17 @@ def _updated_slots(model, active: Optional[torch.Tensor]):
 
 
 def optimizer_state_to_torch(model, opt: Optimizer, flat_state: Dict[str, torch.Tensor],
-                             active: Optional[torch.Tensor] = None, step: int = 0) -> dict:
+                             active: Optional[torch.Tensor] = None, step: int = 0,
+                             pretrain: Optional[torch.Tensor] = None) -> dict:
     """What ``torch.optim.SGD`` / ``Adam(model.parameters(), ...)`` with ``opt``'s hyper-parameters (main.py:83 / 86)
     returns from ``state_dict()`` when its state is that of the flat buffers ``flat_state`` (by torch's state name:
     'momentum_buffer', or 'exp_avg' and 'exp_avg_sq'; laid out as ``bucket_layout``).  One param group listing every
     parameter of the model; state only for the parameters ``active`` lets the update touch, keyed by their index in
     ``model.parameters()``.  ``step``: the Adam step count, for SGD any positive number once an update has run; 0
     means no update yet, and the state is empty, as torch's is before its first step.  The state tensors are copies
-    that own their storage (a view would save the whole flat buffer and follow later steps).  Works on CPU tensors."""
+    that own their storage (a view would save the whole flat buffer and follow later steps).  Works on CPU tensors.
+    ``pretrain``: the per-element mask of the source-only pre-training update (``TrainStep(pretrain_source=True)``);
+    its parameters are updated twice per iteration, so torch.optim.Adam holds step 2 * ``step`` for them."""
     # the param group as the installed torch writes it, from a stock optimizer over one host tensor (a torch.optim
     # optimizer is freed by the cyclic garbage collector only: one over the model would keep the exported state's
     # device memory alive until that runs)
@@ -288,14 +292,21 @@ def optimizer_state_to_torch(model, opt: Optimizer, flat_state: Dict[str, torch.
     state = {}
     if step > 0:
         keys = _state_keys(opt)
+        twice = _pretrain_indices(model, pretrain)
         for i, p, off in sorted(_updated_slots(model, active), key=lambda s: s[0]):
             entry = {k: flat_state[k][off:off + p.numel()].view_as(p).clone() for k in keys}
             if isinstance(opt, Adam):
                 # torch.optim.Adam's step: a 0-dim float tensor on the host (non-capturable, non-fused path)
                 dtype = torch.float64 if torch.get_default_dtype() == torch.float64 else torch.float32
-                entry = {"step": torch.tensor(float(step), dtype=dtype), **entry}
+                t = 2 * step if i in twice else step
+                entry = {"step": torch.tensor(float(t), dtype=dtype), **entry}
             state[i] = entry
     return {"state": state, "param_groups": [group]}
+
+
+def _pretrain_indices(model, pretrain: Optional[torch.Tensor]) -> set:
+    """Indices in ``model.parameters()`` of the tensors the pre-training update touches (``pretrain``: its mask)."""
+    return set() if pretrain is None else {i for i, _, _ in _updated_slots(model, pretrain)}
 
 
 # switches that only some torch releases write into a param group; a group without one had it off
@@ -306,7 +317,8 @@ _SGD_FIXED = {"dampening": 0, "nesterov": True, "maximize": False}
 
 
 def optimizer_state_from_torch(model, opt: Optimizer, sd: dict, flat_state: Dict[str, torch.Tensor],
-                               active: Optional[torch.Tensor] = None) -> Tuple[float, int]:
+                               active: Optional[torch.Tensor] = None,
+                               pretrain: Optional[torch.Tensor] = None) -> Tuple[float, int]:
     """Copy a torch.optim ``state_dict()`` -- from ``optimizer_state_to_torch`` or from a stock SGD / Adam built over
     ``model.parameters()`` -- into the flat buffers ``flat_state`` in place, after checking that the fused update can
     continue it.  Raises ValueError for: another optimizer type (a param group whose keys are not those torch.optim.SGD
@@ -315,7 +327,9 @@ def optimizer_state_from_torch(model, opt: Optimizer, sd: dict, flat_state: Dict
     decay); Adam step counts that differ between parameters, or Adam state missing for some updated parameter; state
     for a parameter the update never touches; a state tensor of the wrong shape.  Nothing is written unless every
     check passes.  Returns (lr, step): step is the Adam step count, for SGD 1 when the dict carries state, else 0.  A
-    parameter without SGD momentum gets a zero buffer, which is what torch's first step does (its buffer = d)."""
+    parameter without SGD momentum gets a zero buffer, which is what torch's first step does (its buffer = d).
+    ``pretrain`` (the mask of ``optimizer_state_to_torch``): the Adam steps must be 2k for the parameters it marks and
+    k for the others, the counts of a run with main.py's --pretrain_source after k iterations; step is then k."""
     groups = sd.get("param_groups") if isinstance(sd, dict) else None
     if not isinstance(groups, (list, tuple)) or len(groups) != 1:
         raise ValueError("the fused update runs one parameter group; the state_dict must have exactly one")
@@ -352,6 +366,7 @@ def optimizer_state_from_torch(model, opt: Optimizer, sd: dict, flat_state: Dict
     keys = _state_keys(opt)
     state = sd.get("state", {})
     steps = set()
+    twice = _pretrain_indices(model, pretrain)
     for i, entry in state.items():
         if i not in slots:
             raise ValueError(f"state for parameter {i}, which the fused update never touches (it gets no gradient)")
@@ -364,9 +379,13 @@ def optimizer_state_from_torch(model, opt: Optimizer, sd: dict, flat_state: Dict
             if not torch.is_tensor(t) or tuple(t.shape) != tuple(p.shape):
                 raise ValueError(f"state[{i}][{k!r}] is not a tensor of shape {tuple(p.shape)}")
         if is_adam:
-            steps.add(float(entry["step"]))
+            steps.add(float(entry["step"]) / (2 if i in twice else 1))
     step = 1 if state else 0
     if is_adam and state:
+        if pretrain is not None and (len(steps) != 1 or len(state) != len(slots)):
+            raise ValueError("with the source-only pre-training update the parameters it reaches take two Adam steps "
+                             "per iteration: the state must hold every parameter the update touches, with step 2k "
+                             "for those and k for the others")
         if len(steps) != 1 or len(state) != len(slots):
             raise ValueError("the fused Adam update keeps one step count for every parameter it touches: the state "
                              "must hold every one of them, with equal steps")
@@ -399,7 +418,7 @@ class TrainStep:
                  class_weight: Optional[torch.Tensor] = None, domain_weight: Sequence[float] = (1.0, 1.0),
                  allreduce: Optional[str] = None, mu: float = 0.0, sampler=None, stats: bool = False,
                  stats_topk: Sequence[int] = (1, 5), dis_DA: str = "none", alpha: float = 0.0,
-                 place_dis: Sequence[str] = ("Y", "Y", "N")):
+                 place_dis: Sequence[str] = ("Y", "Y", "N"), pretrain_source: bool = False):
         """mode: 'legacy' (default) = the per-operator sequence (25 launches in one CUDA graph; the only mode that
         supports use_attn_frame); 'phased' = the step program as 14 launches (ta3n_step_run_phased; default when class /
         domain weights or a scheduled beta are given).  class_weight / domain_weight: the weights of criterion /
@@ -453,7 +472,16 @@ class TrainStep:
         rows' class logits (main.py:541-545, loss.py:8-12), one launch after the loss launches
         (``ta3n_target_entropy_fwd_bwd``); a batch with no real target row contributes 0.  Under MCD it reads pass 1's
         target logits (main.py:542 runs before the reverse pass).  With stats=True the ``loss`` meter includes gamma *
-        the term and ``TrainStats.loss_e`` holds the term, n = the real target rows (main.py:544)."""
+        the term and ``TrainStats.loss_e`` holds the term, n = the real target rows (main.py:544).
+
+        pretrain_source (mode 'legacy', single rank, needs an optimizer; class / domain weights and a negative beta are
+        refused): main.py:388-414 with --pretrain_source, in the same graph ahead of the adaptation pass.  A forward of
+        the source rows only, with dropout masks of its own, CE(out_s) (+ CE(out_s_2) under MCD), its backward into the
+        gradient bucket, clip_grad_norm_ and the optimizer over the parameters that loss reaches (P: the shared layers,
+        the TRN, the classifier(s), the relation discriminators under use_attn and the frame discriminator under frame
+        attention; torch.optim skips the others, whose .grad is None).  Then the adaptation iteration above runs on the
+        updated weights.  ``loss``, the meters and the gradients left in ``.grad`` are the adaptation pass's; Adam
+        counts two steps per iteration for P's parameters and one for the others, as torch.optim.Adam does."""
         if optimizer is not None and not isinstance(optimizer, (SGDNesterov, Adam)):
             raise TypeError(f"optimizer must be SGDNesterov or Adam, got {type(optimizer).__name__}")
         if isinstance(optimizer, Adam):
@@ -525,6 +553,23 @@ class TrainStep:
             mode = "legacy"
         elif float(alpha) != 0.0:
             raise ValueError("alpha weights the discrepancy loss (dis_DA='DAN' / 'JAN'); without it it does nothing")
+        self.pretrain = bool(pretrain_source)
+        if self.pretrain:
+            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
+                raise NotImplementedError("pretrain_source runs in mode='legacy' only (the step program has one "
+                                          "update per iteration)")
+            if class_weight is not None or any(float(b) < 0 for b in beta) or \
+                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
+                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
+                                          "(mode='phased'), which does not cover pretrain_source")
+            if (dist.get_world_size(process_group) if dist.is_initialized() else 1) > 1:
+                # the pre-training update would need an all-reduce of its own before it is applied, and the peer
+                # all-reduce takes the step counter as a once-per-step sequence number
+                raise NotImplementedError("pretrain_source runs on a single rank")
+            if optimizer is None:
+                raise ValueError("pretrain_source is an optimizer step before each adaptation step (main.py:408-414): "
+                                 "it needs TrainStep(optimizer=SGDNesterov(...) or Adam(...))")
+            mode = "legacy"
         self.model = model
         self.params = step_parameters(model)
         self.n_path = len(model.path_parameters())     # the path operators' tensors; MCD's second classifier follows
@@ -683,6 +728,8 @@ class TrainStep:
             add_fc=self.add_fc, drop_stack=self._stack_drops(seed, di))
         if self.mcd:
             self._init_mcd(seed, di, dv, offs)
+        if self.pretrain:
+            self._init_pretrain(seed, di, dv, offs)
         self._init_stats(stats, stats_topk)
         self._init_dis(dis_DA, alpha, place_dis)
         if self.target_entropy and self.mcd and self.pred_video_t1 is None:
@@ -935,6 +982,85 @@ class TrainStep:
         lo, hi = self.acc_range
         check(lib.ta3n_accumulate(_P(self.flat_grad[lo:]), _P(self.flat_grad2[lo:]), hi - lo, st))
 
+    def _init_pretrain(self, seed, di, dv, offs):
+        """State of the source-only pre-training update: its dropout seeds, buffers, the mask of the parameters its
+        loss reaches (P), the bucket ranges outside P and, under Adam, the step count of P's parameters."""
+        dev, f32 = self.device, dict(device=self.device, dtype=torch.float32)
+        Bs, C, R = self.Bs, self.C, self.R
+        s = (seed ^ _PRETRAIN_KEY) & (2 ** 63 - 1)
+        self.pretrain_seeds = (s, s ^ 0x9E3779B9)      # (drop_i, drop_v), keyed by the same step counter
+        # CE on the class logits only: no video discriminator, and the frame discriminator only under frame attention
+        self.spec_pre = TF.PathSpec(
+            num_segments=self.T, beta=self.spec.beta, mu=0.0, reverse=False, use_attn=self.spec.use_attn,
+            use_attn_frame=self.spec.use_attn_frame, classify_only=True,
+            drop_i=TF.DropSpec(p=di, seed=s, step=self.step_counter) if di > 0 else TF.DropSpec(),
+            drop_v=TF.DropSpec(p=dv, seed=s ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec(),
+            add_fc=self.add_fc, drop_stack=self._stack_drops(s, di))
+        self.bufs_pre = TF.Buffers(dev, persistent=True)
+        self.x_none = torch.zeros(0, self.T, self.D, **f32)            # the pass has no target half
+        self.loss_pre = torch.zeros(1, **f32)
+        self.g_video_pre = torch.zeros(Bs, C, **f32)
+        if self.mcd:
+            self.pred2_pre, self.g_video2_pre = torch.zeros(Bs, C, **f32), torch.zeros(Bs, C, **f32)
+        # P: CE reaches the relation discriminators through the attention weights and the frame discriminator through
+        # the frame attention; it never reaches the video discriminator
+        cls = 6 + 6 * R
+        outside = list(range(cls + 2, cls + 6))
+        if not self.spec.use_attn:
+            outside += list(range(6 + 2 * R, cls))
+        if not self.spec.use_attn_frame:
+            outside += [2, 3, 4, 5]
+        size = lambda i: -(-self.params[i].numel() // _ALIGN) * _ALIGN      # noqa: E731
+        self.pretrain_mask = torch.ones_like(self.flat_grad)
+        ranges = []
+        for i in sorted(outside, key=lambda i: offs[i]):
+            lo, hi = offs[i], offs[i] + size(i)
+            self.pretrain_mask[lo:hi] = 0.0
+            if ranges and ranges[-1][1] == lo:
+                ranges[-1] = (ranges[-1][0], hi)
+            else:
+                ranges.append((lo, hi))
+        # the backward does not write these slots, which still hold the previous adaptation pass's gradient: the
+        # clip's norm runs over the whole bucket
+        self.pretrain_stale = [self.flat_grad[lo:hi] for lo, hi in ranges]
+        # Adam: the adaptation pass updates P with P's step count and the rest of its set (P lies inside it) with the
+        # other one
+        rest = (self.active_mask if self.active_mask is not None else torch.ones_like(self.flat_grad)) - \
+            self.pretrain_mask
+        self.pretrain_rest = rest if bool((rest != 0).any()) else None
+        if isinstance(self.opt, Adam):
+            self.adam_step_pre = torch.zeros(1, device=dev, dtype=torch.int64)
+
+    def _enqueue_pretrain(self, lib, st, optimizer):
+        """The pre-training update (main.py:388-414): the source rows' forward, CE (+ CE of the second classifier),
+        the backward into the gradient bucket, the slots outside P zeroed, then clip + the optimizer over P."""
+        Bs, C = self.Bs, self.C
+        saved, outputs, dims = TF.path_forward(self.spec_pre, self.xs, self.x_none, self.params[:self.n_path],
+                                               self.bufs_pre, batch_gemms=True)
+        self.loss_pre.zero_()
+        check(lib.ta3n_ce_loss_fwd_bwd(_P(outputs[5]), _P(self.labels), Bs, C, _P(self.valid), _P(self.loss_pre),
+                                       _P(self.g_video_pre), st))
+        gin = {"pred_video": self.g_video_pre}
+        check(lib.ta3n_wgrad_defer_begin())
+        if self.mcd:
+            w2, b2 = self.params[-2], self.params[-1]
+            check(lib.ta3n_video_head_fwd(_P(saved["dropped"]), Bs, w2.shape[1], C, _P(w2), _P(b2), None,
+                                          _P(self.head2_scratch), _P(self.pred2_pre), st))
+            check(lib.ta3n_ce_loss_fwd_bwd(_P(self.pred2_pre), _P(self.labels), Bs, C, _P(self.valid),
+                                           _P(self.loss_pre), _P(self.g_video2_pre), st))
+            d_dropped = self.bufs_pre.get("d_dropped", Bs, w2.shape[1])
+            self._enqueue_head2_bwd(lib, st, self.bufs_pre, saved["dropped"], Bs, self.g_video2_pre, d_dropped,
+                                    self.grad_views)
+            gin["dropped"] = d_dropped
+        TF.path_backward(self.spec_pre, dims, self.xs, self.x_none, self.params[:self.n_path], saved, gin,
+                         self.grad_views[:self.n_path], self.bufs_pre)
+        ws = self.bufs_pre.workspace("wgrad", lib.ta3n_wgrad_defer_workspace_bytes())
+        check(lib.ta3n_wgrad_defer_flush(_P(ws), ws.numel(), st))
+        for t in self.pretrain_stale:
+            t.zero_()
+        if optimizer:
+            self._launch_optimizer(self.pretrain_mask, getattr(self, "adam_step_pre", None))
+
     # -- gradient bucket / all-reduce ------------------------------------------------------------------
     def _alloc_gradient_bucket(self, n, allreduce):
         """The flat gradient bucket.  With several ranks it is allocated in SYMMETRIC memory (same size on every rank,
@@ -1081,20 +1207,37 @@ class TrainStep:
     # -- the fixed launch sequence ---------------------------------------------------------------------
     def _enqueue_optimizer(self):
         """clip_grad_norm_ + SGD-Nesterov or Adam over the flat buffers (main.py:578-583): two launches (one without
-        clipping)."""
+        clipping).  With pretrain_source, Adam runs as two such updates: P with P's step count, then the rest of the
+        set with its own; both fold the clip coefficient from the same whole-bucket norm."""
+        if self.pretrain and isinstance(self.opt, Adam):
+            self._launch_optimizer(self.pretrain_mask, self.adam_step_pre)
+            if self.pretrain_rest is not None:
+                self._launch_optimizer(self.pretrain_rest, self.adam_step)
+            return
+        self._launch_optimizer(self.active_mask, getattr(self, "adam_step", None))
+
+    def _optimizer_launches(self) -> int:
+        """Launches of the optimizer updates of one iteration (those of the pre-training update included)."""
+        calls = 1
+        if self.pretrain:
+            calls = 2 + (1 if isinstance(self.opt, Adam) and self.pretrain_rest is not None else 0)
+        return calls * (2 if self.opt.clip_gradient is not None else 1)
+
+    def _launch_optimizer(self, mask, adam_step):
+        """One clip + update over the elements ``mask`` marks (None: all); ``adam_step``: the Adam step count."""
         o = self.opt
         clip = float(o.clip_gradient) if o.clip_gradient is not None else 0.0
         if isinstance(o, Adam):
             check(_lib.load().ta3n_adam_step_masked(
                 _P(self.flat_param), _P(self.flat_grad), _P(self.exp_avg), _P(self.exp_avg_sq), self.flat_grad.numel(),
-                _P(self.lr_dev), _P(self.adam_step), float(o.betas[0]), float(o.betas[1]), float(o.eps),
+                _P(self.lr_dev), _P(adam_step), float(o.betas[0]), float(o.betas[1]), float(o.eps),
                 float(o.weight_decay), clip, _P(self.opt_ws), self.opt_ws.numel() * 4, _P(self.grad_stats),
-                _P(self.active_mask), TF._stream()))
+                _P(mask), TF._stream()))
             return
         check(_lib.load().ta3n_sgd_nesterov_step_masked(
             _P(self.flat_param), _P(self.flat_grad), _P(self.momentum_buf), self.flat_grad.numel(),
             _P(self.lr_dev), float(o.momentum), float(o.weight_decay), clip, _P(self.opt_ws),
-            self.opt_ws.numel() * 4, _P(self.grad_stats), _P(self.active_mask), TF._stream()))
+            self.opt_ws.numel() * 4, _P(self.grad_stats), _P(mask), TF._stream()))
 
     def set_lr(self, lr: float):
         """Per-step learning-rate schedules (main.py:800-802): one 4-byte fill on the stream, no re-capture."""
@@ -1115,8 +1258,16 @@ class TrainStep:
         (``'optimizer': optimizer.state_dict()``, main.py:266-274) keeps its format.  Synchronises with the device."""
         if self.opt is None:
             raise ValueError("optimizer_state_dict needs TrainStep(optimizer=...)")
-        step = int(self.adam_step.item()) if isinstance(self.opt, Adam) else int(self._opt_stepped)
-        return optimizer_state_to_torch(self.model, self.opt, self._flat_state(), self.active_mask, step)
+        if isinstance(self.opt, Adam):
+            # with pretrain_source P's count is 2k after k iterations (the rest of the set may be empty)
+            step = int(self.adam_step_pre.item()) // 2 if self.pretrain else int(self.adam_step.item())
+        else:
+            step = int(self._opt_stepped)
+        return optimizer_state_to_torch(self.model, self.opt, self._flat_state(), self.active_mask, step,
+                                        self._pretrain_mask())
+
+    def _pretrain_mask(self):
+        return self.pretrain_mask if self.pretrain else None
 
     def load_optimizer_state_dict(self, sd: dict) -> None:
         """Continue from a torch.optim ``state_dict()`` -- this class's, or a stock SGD / Adam's built over
@@ -1125,10 +1276,13 @@ class TrainStep:
         ValueError when the update cannot continue it (``optimizer_state_from_torch``)."""
         if self.opt is None:
             raise ValueError("load_optimizer_state_dict needs TrainStep(optimizer=...)")
-        lr, step = optimizer_state_from_torch(self.model, self.opt, sd, self._flat_state(), self.active_mask)
+        lr, step = optimizer_state_from_torch(self.model, self.opt, sd, self._flat_state(), self.active_mask,
+                                              self._pretrain_mask())
         self.set_lr(lr)
         if isinstance(self.opt, Adam):
             self.adam_step.fill_(step)
+            if self.pretrain:
+                self.adam_step_pre.fill_(2 * step)
         self._opt_stepped = step > 0
 
     def state_dict(self) -> dict:
@@ -1182,6 +1336,8 @@ class TrainStep:
             self._join_stats()
             return
         check(lib.ta3n_counter_inc(_P(self.step_counter), st))          # fresh dropout masks per step
+        if self.pretrain:
+            self._enqueue_pretrain(lib, st, optimizer and self.opt is not None)
         saved, outputs, dims = TF.path_forward(self.spec, self.xs, self.xt, self.params[:self.n_path], self.bufs,
                                                batch_gemms=True)
         self.outputs = outputs
@@ -1301,7 +1457,7 @@ class TrainStep:
                 self._enqueue(at_split=(lambda: None) if self.split else None)   # warm-up: sizes every buffer
             self.launches_per_step = _lib.launch_count() - n0        # warm-up never applies the optimizer
             if self.opt is not None:
-                self.launches_per_step += 2 if self.opt.clip_gradient is not None else 1
+                self.launches_per_step += self._optimizer_launches()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         if self.world > 1 and self.split and self.graph_collectives:
