@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define TA3N_ABI_VERSION 7
+#define TA3N_ABI_VERSION 8
 
 enum {
   TA3N_OK = 0,
@@ -265,6 +265,15 @@ int ta3n_loss_fwd_bwd(const float* pred_video, const long long* labels, const fl
                       float* g_pred_video,
                       float* g_pred_rel, float* g_pred_dom_video, float* g_pred_frame,
                       void* workspace, size_t workspace_bytes, ta3n_stream_t stream);
+/* The same launches with target labels (use_target='Sv', main.py:442-446): the class CE runs over the real source
+ * rows AND the real target rows, target row r against labels_t[r] (int64, [Bt]), with its mean and gradient over
+ * vs + vt rows instead of vs.  Every other term is as above; padded rows get zero loss and gradient, and vt = 0 gives
+ * the source-only mean.  labels_t must not be NULL (ta3n_loss_fwd_bwd is the call without target labels).          */
+int ta3n_loss_fwd_bwd_sv(const float* pred_video, const long long* labels, const long long* labels_t,
+                         const float* pred_rel, const float* pred_dom_video, const float* pred_frame, int Bs, int Bt,
+                         int T, int R, int C, float gamma, int flags, const int* valid_rows, float* loss,
+                         float* g_pred_video, float* g_pred_rel, float* g_pred_dom_video, float* g_pred_frame,
+                         void* workspace, size_t workspace_bytes, ta3n_stream_t stream);
 /* *counter += 1 on the stream (dropout step counter for CUDA-graph replays). */
 int ta3n_counter_inc(uint64_t* counter, ta3n_stream_t stream);
 
@@ -335,6 +344,14 @@ int ta3n_gather_batch(const float* bank_s, long long n_rows_s, const int* rows_s
                       long long n_epoch_s, int batch_s, float* x_s, long long* y_s,
                       const float* bank_t, long long n_rows_t, const int* rows_t, long long n_epoch_t, int batch_t,
                       float* x_t, long long row_floats, int* valid_rows, unsigned int* state, ta3n_stream_t stream);
+/* ta3n_gather_batch with the target labels as well (use_target='Sv'): labels_t [n_epoch_t] int64 is the target label
+ * list and y_t [batch_t] int64 the target slot labels, filled like the source ones (padded rows get label 0).  Same
+ * launch, same kernel label; ta3n_gather_batch is this call with no target label list.                             */
+int ta3n_gather_batch_labelled(const float* bank_s, long long n_rows_s, const int* rows_s, const long long* labels_s,
+                               long long n_epoch_s, int batch_s, float* x_s, long long* y_s,
+                               const float* bank_t, long long n_rows_t, const int* rows_t, const long long* labels_t,
+                               long long n_epoch_t, int batch_t, float* x_t, long long* y_t, long long row_floats,
+                               int* valid_rows, unsigned int* state, ta3n_stream_t stream);
 /* The same gather for ONE labelled domain in a fixed order (validation: main.py:178 uses shuffle=False; the row list
  * carries the num_dataload tiling): the rows of epoch positions [i*batch, min((i+1)*batch, n_epoch)) go to x
  * [batch, row_floats], their labels to y [batch], the rest is zero-filled with label 0, valid_rows [1] = the number of
@@ -425,6 +442,21 @@ int ta3n_train_stats_accumulate(const float* pred_video, const long long* labels
                                 int flags, const int* valid_rows, const float* class_weight,
                                 const float* domain_weight_host, int n_k, const int* k_host, ta3n_train_stats* accum,
                                 void* workspace, size_t workspace_bytes, ta3n_stream_t stream);
+
+/* The meters with target labels (use_target='Sv'), as ta3n_train_stats_accumulate except:
+ *   loss_c  val = the class CE over the vs + vt real rows, target row r against labels_t[r]; n = vs (main.py:446-450);
+ *   top-k   the hits over the vs + vt real rows: correct / correct_step / rows / rows_step of *accum count them, and
+ *           main.py:565-571 folds accuracy() (percent over vs + vt rows) with n = vs, which integer counts cannot
+ *           express when the last batch is short: prec_sum[q] (fp64, one per k, zero it with *accum) gets
+ *           += 100 * hits_q / (vs + vt) * vs.  The meter's average is prec_sum[q] / count[1] (loss_c's n, also vs).
+ * MCD's second classifier is not taken (pred2_s / pred2_t NULL): the reference fails on it under Sv (main.py:448).
+ * labels_t and prec_sum must not be NULL; prec_sum 8-byte aligned.  Kernel label "train_stats".                   */
+int ta3n_train_stats_accumulate_sv(const float* pred_video, const long long* labels, const long long* labels_t,
+                                   const float* pred_rel, const float* pred_dom_video, const float* pred_frame,
+                                   const float* loss, int Bs, int Bt, int T, int R, int C, int flags,
+                                   const int* valid_rows, const float* class_weight, const float* domain_weight_host,
+                                   int n_k, const int* k_host, ta3n_train_stats* accum, double* prec_sum,
+                                   void* workspace, size_t workspace_bytes, ta3n_stream_t stream);
 
 /* ---- the training step as one step program (SURVEY 8a rows a1-a13 + 8f row n1) ----------------------------- */
 /* main.py:418 (model forward, models.py:545-722 trn-m branch), main.py:446, 508-538, 559-562 (composed loss:

@@ -11,7 +11,7 @@ import threading
 
 from . import build as _build
 
-ABI_VERSION = 7     # TA3N_ABI_VERSION of include/ta3n_b200.h that SIGNATURES mirrors
+ABI_VERSION = 8     # TA3N_ABI_VERSION of include/ta3n_b200.h that SIGNATURES mirrors
 
 TA3N_GEMM_FP32_SIMT = 0
 TA3N_GEMM_TF32_TCGEN05 = 1
@@ -103,6 +103,8 @@ SIGNATURES = {
     "ta3n_loss_workspace_bytes": (_SZ, [_I]),
     "ta3n_loss_fwd_bwd": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _F, _I, _VP, _VP, _VP, _VP, _VP, _VP,
                                _VP, _SZ, _VP]),
+    "ta3n_loss_fwd_bwd_sv": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _F, _I, _VP, _VP, _VP, _VP, _VP,
+                                  _VP, _VP, _SZ, _VP]),
     "ta3n_counter_inc": (_I, [_VP, _VP]),
     "ta3n_ce_loss_fwd_bwd": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP]),
     "ta3n_mcd_loss_fwd_bwd": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
@@ -113,6 +115,8 @@ SIGNATURES = {
                                       _I, _VP, _VP, _VP, _VP, _VP, _VP, _SZ, _VP]),
     "ta3n_gather_batch": (_I, [_VP, C.c_longlong, _VP, _VP, C.c_longlong, _I, _VP, _VP,
                                _VP, C.c_longlong, _VP, C.c_longlong, _I, _VP, C.c_longlong, _VP, _VP, _VP]),
+    "ta3n_gather_batch_labelled": (_I, [_VP, C.c_longlong, _VP, _VP, C.c_longlong, _I, _VP, _VP, _VP, C.c_longlong,
+                                        _VP, _VP, C.c_longlong, _I, _VP, _VP, C.c_longlong, _VP, _VP, _VP]),
     "ta3n_gather_rows": (_I, [_VP, C.c_longlong, _VP, _VP, C.c_longlong, _I, _VP, _VP, C.c_longlong, _VP, _VP, _VP]),
     "ta3n_eval_workspace_bytes": (_SZ, [_I]),
     "ta3n_eval_head": (_I, [_VP, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _I, _IP, _VP, _I, C.c_longlong, _VP,
@@ -120,6 +124,8 @@ SIGNATURES = {
     "ta3n_train_stats_workspace_bytes": (_SZ, [_I]),
     "ta3n_train_stats_accumulate": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP, _VP,
                                          C.POINTER(C.c_float), _I, _IP, _VP, _VP, _SZ, _VP]),
+    "ta3n_train_stats_accumulate_sv": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP, _VP,
+                                            C.POINTER(C.c_float), _I, _IP, _VP, _VP, _VP, _SZ, _VP]),
     "ta3n_step_workspace_bytes": (_SZ, [C.POINTER(StepDesc)]),
     "ta3n_step_run_phased": (_I, [C.POINTER(StepDesc), _VP]),
     "ta3n_allreduce_flag_bytes": (_SZ, [_I]),

@@ -597,7 +597,7 @@ enum : int { LOSS_ADV_REL = 1, LOSS_ADV_VIDEO = 2, LOSS_ADV_FRAME = 4, LOSS_ATT_
 
 __global__ void __launch_bounds__(256)
 loss_heads_kernel(const float* __restrict__ pred_video, const long long* __restrict__ labels,
-                  const float* __restrict__ pred_rel, const float* __restrict__ pred_dom,
+                  const long long* __restrict__ labels_t, const float* __restrict__ pred_rel, const float* __restrict__ pred_dom,
                   const float* __restrict__ pred_frame, int Bs, int M, int T, int R, int C, float gamma, int flags,
                   const int* __restrict__ valid_rows, float* __restrict__ g_video, float* __restrict__ g_rel,
                   float* __restrict__ g_dom, float* __restrict__ g_frame, float* __restrict__ row_loss) {
@@ -610,6 +610,9 @@ loss_heads_kernel(const float* __restrict__ pred_video, const long long* __restr
   const int vs = valid_rows ? min(valid_rows[0], Bs) : Bs;
   const int vt = valid_rows ? min(valid_rows[1], M - Bs) : M - Bs;
   const float n_src = (float)max(vs, 1), n_all = (float)max(vs + vt, 1);
+  // labels_t (use_target='Sv', main.py:442-446): the class CE also covers the target rows, its mean over vs + vt
+  const bool sv = labels_t != nullptr;
+  const float n_cls = sv ? n_all : n_src;
   for (int m = blockIdx.x * warps_per_block + (threadIdx.x >> 5); m < M; m += gridDim.x * warps_per_block) {
     const int dom = m >= Bs ? 1 : 0;
     if (dom ? (m - Bs >= vt) : (m >= vs)) {   // padding row
@@ -641,15 +644,16 @@ loss_heads_kernel(const float* __restrict__ pred_video, const long long* __restr
     const Attn2 dv = attn_from_logits(pred_dom[(size_t)m * 2], pred_dom[(size_t)m * 2 + 1]);
     const bool att = (flags & LOSS_ATT_ENT) != 0;
     const float att_scale = att ? gamma / n_all : 0.f;
-    const long long y = (m < Bs) ? labels[m] : -1;
+    const bool labelled = m < Bs || sv;
+    const long long y = (m < Bs) ? labels[m] : (sv ? labels_t[m - Bs] : -1);
     for (int c = lane; c < C; c += 32) {
       const float lq = pv[c] - mx - lse;
       const float q = expf(lq);
       float gq = 0.f;
-      if (m < Bs) gq = (q - (c == (int)y ? 1.f : 0.f)) / n_src;
+      if (labelled) gq = (q - (c == (int)y ? 1.f : 0.f)) / n_cls;
       gq += att_scale * (1.f + dv.ent) * (-q * (lq + hc));
       g_video[(size_t)m * C + c] = gq;
-      if (m < Bs && c == (int)y && lane == (c & 31)) loss += -lq / n_src;
+      if (labelled && c == (int)y && lane == (c & 31)) loss += -lq / n_cls;
     }
     loss = warp_sum(loss);   // exactly one lane held the CE term
     if (lane == 0) {

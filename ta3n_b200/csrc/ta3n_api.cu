@@ -985,26 +985,54 @@ int ta3n_video_head_bwd(const float* dropped, int M, int H, int C, const float* 
 // ------------------------------------------------------------------------------------------------
 size_t ta3n_loss_workspace_bytes(int M) { return Arena::round((size_t)M * sizeof(float)) + 256; }
 
-int ta3n_loss_fwd_bwd(const float* pred_video, const long long* labels, const float* pred_rel,
-                      const float* pred_dom_video, const float* pred_frame, int Bs, int Bt, int T, int R, int C,
-                      float gamma, int flags, const int* valid_rows, float* loss, float* g_pred_video,
-                      float* g_pred_rel, float* g_pred_dom_video, float* g_pred_frame, void* workspace,
-                      size_t workspace_bytes, ta3n_stream_t stream) {
-  TA3N_REQUIRE(Bs >= 1 && Bt >= 0 && T >= 1 && R >= 1 && C >= 1, "bad sizes");
-  TA3N_REQUIRE(pred_video && labels && pred_rel && pred_dom_video && pred_frame && loss, "null input");
-  TA3N_REQUIRE(g_pred_video && g_pred_rel && g_pred_dom_video && g_pred_frame, "null gradient output");
+// TA3N_REQUIRE for helpers behind several entry points: the message names the entry (`who`), not the helper
+#define TA3N_REQUIRE_WHO(cond, msg)                                                                         \
+  do {                                                                                                     \
+    if (!(cond)) return fail(TA3N_ERR_INVALID, "%s: requirement failed: " msg " (line %d)", who, (int)__LINE__); \
+  } while (0)
+
+// labels_t == nullptr: the shipped loss (ta3n_loss_fwd_bwd); otherwise the class CE covers the target rows (Sv)
+static int loss_heads(const char* who, const float* pred_video, const long long* labels, const long long* labels_t,
+                      const float* pred_rel, const float* pred_dom_video, const float* pred_frame, int Bs, int Bt,
+                      int T, int R, int C, float gamma, int flags, const int* valid_rows, float* loss,
+                      float* g_pred_video, float* g_pred_rel, float* g_pred_dom_video, float* g_pred_frame,
+                      void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
+  TA3N_REQUIRE_WHO(Bs >= 1 && Bt >= 0 && T >= 1 && R >= 1 && C >= 1, "bad sizes");
+  TA3N_REQUIRE_WHO(pred_video && labels && pred_rel && pred_dom_video && pred_frame && loss, "null input");
+  TA3N_REQUIRE_WHO(g_pred_video && g_pred_rel && g_pred_dom_video && g_pred_frame, "null gradient output");
   const int M = Bs + Bt;
   Arena arena(workspace, workspace_bytes);
   float* row_loss = arena.floats(M);
-  if (!row_loss) return fail(TA3N_ERR_WORKSPACE, "ta3n_loss_fwd_bwd: workspace too small (%zu bytes)", workspace_bytes);
+  if (!row_loss) return fail(TA3N_ERR_WORKSPACE, "%s: workspace too small (%zu bytes)", who, workspace_bytes);
   pre_launch("loss_heads", S(stream));
   launch_kernel(loss_heads_kernel, blocks_for((size_t)M * 32, 256), 256, 0, S(stream), 
-      pred_video, labels, pred_rel, pred_dom_video, pred_frame, Bs, M, T, R, C, gamma, flags, valid_rows,
+      pred_video, labels, labels_t, pred_rel, pred_dom_video, pred_frame, Bs, M, T, R, C, gamma, flags, valid_rows,
       g_pred_video, g_pred_rel, g_pred_dom_video, g_pred_frame, row_loss);
   TA3N_TRY(after_launch());
   pre_launch("loss_reduce", S(stream));
   launch_kernel(loss_reduce_kernel, 1, 1024, 0, S(stream), row_loss, M, loss);
   return after_launch();
+}
+
+int ta3n_loss_fwd_bwd(const float* pred_video, const long long* labels, const float* pred_rel,
+                      const float* pred_dom_video, const float* pred_frame, int Bs, int Bt, int T, int R, int C,
+                      float gamma, int flags, const int* valid_rows, float* loss, float* g_pred_video,
+                      float* g_pred_rel, float* g_pred_dom_video, float* g_pred_frame, void* workspace,
+                      size_t workspace_bytes, ta3n_stream_t stream) {
+  return loss_heads("ta3n_loss_fwd_bwd", pred_video, labels, nullptr, pred_rel, pred_dom_video, pred_frame, Bs, Bt, T,
+                    R, C, gamma, flags, valid_rows, loss, g_pred_video, g_pred_rel, g_pred_dom_video, g_pred_frame,
+                    workspace, workspace_bytes, stream);
+}
+
+int ta3n_loss_fwd_bwd_sv(const float* pred_video, const long long* labels, const long long* labels_t,
+                         const float* pred_rel, const float* pred_dom_video, const float* pred_frame, int Bs, int Bt,
+                         int T, int R, int C, float gamma, int flags, const int* valid_rows, float* loss,
+                         float* g_pred_video, float* g_pred_rel, float* g_pred_dom_video, float* g_pred_frame,
+                         void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
+  TA3N_REQUIRE(labels_t != nullptr, "null target labels (ta3n_loss_fwd_bwd is the call without them)");
+  return loss_heads("ta3n_loss_fwd_bwd_sv", pred_video, labels, labels_t, pred_rel, pred_dom_video, pred_frame, Bs,
+                    Bt, T, R, C, gamma, flags, valid_rows, loss, g_pred_video, g_pred_rel, g_pred_dom_video,
+                    g_pred_frame, workspace, workspace_bytes, stream);
 }
 
 int ta3n_counter_inc(uint64_t* counter, ta3n_stream_t stream) {
@@ -1130,31 +1158,53 @@ int ta3n_discrepancy_fwd_bwd(int joint, int Bs, int Bt,
 // ------------------------------------------------------------------------------------------------
 // device-resident input pipeline (include/ta3n_b200.h: ta3n_gather_batch)
 // ------------------------------------------------------------------------------------------------
+// labels_t / y_t == nullptr: the target domain carries no labels (ta3n_gather_batch)
+static int gather_batch(const char* who, const float* bank_s, long long n_rows_s, const int* rows_s,
+                        const long long* labels_s, long long n_epoch_s, int batch_s, float* x_s, long long* y_s,
+                        const float* bank_t, long long n_rows_t, const int* rows_t, const long long* labels_t,
+                        long long n_epoch_t, int batch_t, float* x_t, long long* y_t, long long row_floats,
+                        int* valid_rows, unsigned int* state, ta3n_stream_t stream) {
+  TA3N_REQUIRE_WHO(batch_s >= 1 && batch_t >= 1 && batch_s + batch_t <= 65535, "batch sizes must be >= 1, together <= 65535");
+  TA3N_REQUIRE_WHO(row_floats >= 4 && row_floats % 4 == 0, "row_floats must be a positive multiple of 4 (16-byte rows)");
+  TA3N_REQUIRE_WHO(n_epoch_s >= 1 && n_epoch_t >= 1, "empty epoch");
+  TA3N_REQUIRE_WHO(n_rows_s >= 1 && n_rows_t >= 1 && n_rows_s <= INT32_MAX && n_rows_t <= INT32_MAX,
+               "bank rows must be in [1, 2^31) (row lists are int32)");
+  TA3N_REQUIRE_WHO(n_rows_s <= INT64_MAX / row_floats && n_rows_t <= INT64_MAX / row_floats, "bank too large");
+  TA3N_REQUIRE_WHO(bank_s && rows_s && labels_s && x_s && y_s, "null source pointer");
+  TA3N_REQUIRE_WHO(bank_t && rows_t && x_t, "null target pointer");
+  TA3N_REQUIRE_WHO(valid_rows && state, "null valid_rows / state");
+  TA3N_REQUIRE_WHO(aligned16(bank_s) && aligned16(bank_t) && aligned16(x_s) && aligned16(x_t),
+               "banks and slots must be 16-byte aligned");
+  GatherDomain s{reinterpret_cast<const float4*>(bank_s), n_rows_s, rows_s, labels_s, n_epoch_s,
+                 reinterpret_cast<float4*>(x_s), y_s, batch_s};
+  GatherDomain t{reinterpret_cast<const float4*>(bank_t), n_rows_t, rows_t, labels_t, n_epoch_t,
+                 reinterpret_cast<float4*>(x_t), y_t, batch_t};
+  const long long row_f4 = row_floats / 4;
+  const dim3 grid((unsigned)((row_f4 + kGatherChunk - 1) / kGatherChunk), (unsigned)(batch_s + batch_t));
+  TA3N_REQUIRE_WHO(grid.x <= 65535u, "rows too long");
+  pre_launch("gather_batch", S(stream));
+  launch_kernel(gather_batch_kernel, grid, kGatherThreads, 0, S(stream), s, t, row_f4, valid_rows, state);
+  return after_launch();
+}
+
 int ta3n_gather_batch(const float* bank_s, long long n_rows_s, const int* rows_s, const long long* labels_s,
                       long long n_epoch_s, int batch_s, float* x_s, long long* y_s,
                       const float* bank_t, long long n_rows_t, const int* rows_t, long long n_epoch_t, int batch_t,
                       float* x_t, long long row_floats, int* valid_rows, unsigned int* state, ta3n_stream_t stream) {
-  TA3N_REQUIRE(batch_s >= 1 && batch_t >= 1 && batch_s + batch_t <= 65535, "batch sizes must be >= 1, together <= 65535");
-  TA3N_REQUIRE(row_floats >= 4 && row_floats % 4 == 0, "row_floats must be a positive multiple of 4 (16-byte rows)");
-  TA3N_REQUIRE(n_epoch_s >= 1 && n_epoch_t >= 1, "empty epoch");
-  TA3N_REQUIRE(n_rows_s >= 1 && n_rows_t >= 1 && n_rows_s <= INT32_MAX && n_rows_t <= INT32_MAX,
-               "bank rows must be in [1, 2^31) (row lists are int32)");
-  TA3N_REQUIRE(n_rows_s <= INT64_MAX / row_floats && n_rows_t <= INT64_MAX / row_floats, "bank too large");
-  TA3N_REQUIRE(bank_s && rows_s && labels_s && x_s && y_s, "null source pointer");
-  TA3N_REQUIRE(bank_t && rows_t && x_t, "null target pointer");
-  TA3N_REQUIRE(valid_rows && state, "null valid_rows / state");
-  TA3N_REQUIRE(aligned16(bank_s) && aligned16(bank_t) && aligned16(x_s) && aligned16(x_t),
-               "banks and slots must be 16-byte aligned");
-  GatherDomain s{reinterpret_cast<const float4*>(bank_s), n_rows_s, rows_s, labels_s, n_epoch_s,
-                 reinterpret_cast<float4*>(x_s), y_s, batch_s};
-  GatherDomain t{reinterpret_cast<const float4*>(bank_t), n_rows_t, rows_t, nullptr, n_epoch_t,
-                 reinterpret_cast<float4*>(x_t), nullptr, batch_t};
-  const long long row_f4 = row_floats / 4;
-  const dim3 grid((unsigned)((row_f4 + kGatherChunk - 1) / kGatherChunk), (unsigned)(batch_s + batch_t));
-  TA3N_REQUIRE(grid.x <= 65535u, "rows too long");
-  pre_launch("gather_batch", S(stream));
-  launch_kernel(gather_batch_kernel, grid, kGatherThreads, 0, S(stream), s, t, row_f4, valid_rows, state);
-  return after_launch();
+  return gather_batch("ta3n_gather_batch", bank_s, n_rows_s, rows_s, labels_s, n_epoch_s, batch_s, x_s, y_s, bank_t,
+                      n_rows_t, rows_t, nullptr, n_epoch_t, batch_t, x_t, nullptr, row_floats, valid_rows, state,
+                      stream);
+}
+
+int ta3n_gather_batch_labelled(const float* bank_s, long long n_rows_s, const int* rows_s, const long long* labels_s,
+                               long long n_epoch_s, int batch_s, float* x_s, long long* y_s,
+                               const float* bank_t, long long n_rows_t, const int* rows_t, const long long* labels_t,
+                               long long n_epoch_t, int batch_t, float* x_t, long long* y_t, long long row_floats,
+                               int* valid_rows, unsigned int* state, ta3n_stream_t stream) {
+  TA3N_REQUIRE(labels_t && y_t, "null target label list / slot labels (ta3n_gather_batch is the call without them)");
+  return gather_batch("ta3n_gather_batch_labelled", bank_s, n_rows_s, rows_s, labels_s, n_epoch_s, batch_s, x_s, y_s,
+                      bank_t, n_rows_t, rows_t, labels_t, n_epoch_t, batch_t, x_t, y_t, row_floats, valid_rows, state,
+                      stream);
 }
 
 int ta3n_gather_rows(const float* bank, long long n_rows, const int* rows, const long long* labels, long long n_epoch,
@@ -1244,34 +1294,34 @@ size_t ta3n_train_stats_workspace_bytes(int M) {
   return M < 1 ? 0 : Arena::round((size_t)train_stats_grid(M) * sizeof(TrainStatsPartial));
 }
 
-int ta3n_train_stats_accumulate(const float* pred_video, const long long* labels, const float* pred_rel,
-                                const float* pred_dom_video, const float* pred_frame, const float* pred2_s,
-                                const float* pred2_t, const float* loss, int Bs, int Bt, int T, int R, int C,
-                                int flags, const int* valid_rows, const float* class_weight,
-                                const float* domain_weight_host, int n_k, const int* k_host, ta3n_train_stats* accum,
-                                void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
-  TA3N_REQUIRE(accum != nullptr, "null accumulator");
-  TA3N_REQUIRE(reinterpret_cast<uintptr_t>(accum) % 8 == 0, "accum must be 8-byte aligned");
-  TA3N_REQUIRE(Bs >= 1 && Bt >= 0 && T >= 1 && R >= 1 && C >= 1, "bad sizes (M = Bs + Bt must be >= 1, Bs >= 1)");
-  TA3N_REQUIRE((long long)Bs + Bt <= INT32_MAX - kStatsRows, "too many rows");
-  TA3N_REQUIRE(flags >= 0 && flags <= 15, "flags must be a combination of 1, 2, 4 and 8");
-  TA3N_REQUIRE(n_k >= 1 && n_k <= kEvalMaxK && k_host, "between 1 and 4 top-k values");
+static int train_stats(const char* who, const float* pred_video, const long long* labels, const long long* labels_t,
+                       const float* pred_rel, const float* pred_dom_video, const float* pred_frame,
+                       const float* pred2_s, const float* pred2_t, const float* loss, int Bs, int Bt, int T, int R,
+                       int C, int flags, const int* valid_rows, const float* class_weight,
+                       const float* domain_weight_host, int n_k, const int* k_host, ta3n_train_stats* accum,
+                       double* prec_sum, void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
+  TA3N_REQUIRE_WHO(accum != nullptr, "null accumulator");
+  TA3N_REQUIRE_WHO(reinterpret_cast<uintptr_t>(accum) % 8 == 0, "accum must be 8-byte aligned");
+  TA3N_REQUIRE_WHO(Bs >= 1 && Bt >= 0 && T >= 1 && R >= 1 && C >= 1, "bad sizes (M = Bs + Bt must be >= 1, Bs >= 1)");
+  TA3N_REQUIRE_WHO((long long)Bs + Bt <= INT32_MAX - kStatsRows, "too many rows");
+  TA3N_REQUIRE_WHO(flags >= 0 && flags <= 15, "flags must be a combination of 1, 2, 4 and 8");
+  TA3N_REQUIRE_WHO(n_k >= 1 && n_k <= kEvalMaxK && k_host, "between 1 and 4 top-k values");
   for (int i = 0; i < n_k; ++i)
     if (k_host[i] < 1 || k_host[i] > C)
-      return fail(TA3N_ERR_INVALID, "ta3n_train_stats_accumulate: top-k value %d is outside [1, C=%d]", k_host[i], C);
-  TA3N_REQUIRE(pred_video && labels && pred_rel && pred_dom_video && pred_frame && loss, "null input");
-  TA3N_REQUIRE(pred2_s || !pred2_t, "pred2_t without pred2_s (MCD needs both)");
-  TA3N_REQUIRE(!pred2_s || pred2_t || Bt == 0, "pred2_s without pred2_t (MCD needs both when Bt > 0)");
-  TA3N_REQUIRE(domain_weight_host != nullptr, "null domain_weight_host");
+      return fail(TA3N_ERR_INVALID, "%s: top-k value %d is outside [1, C=%d]", who, k_host[i], C);
+  TA3N_REQUIRE_WHO(pred_video && labels && pred_rel && pred_dom_video && pred_frame && loss, "null input");
+  TA3N_REQUIRE_WHO(pred2_s || !pred2_t, "pred2_t without pred2_s (MCD needs both)");
+  TA3N_REQUIRE_WHO(!pred2_s || pred2_t || Bt == 0, "pred2_s without pred2_t (MCD needs both when Bt > 0)");
+  TA3N_REQUIRE_WHO(domain_weight_host != nullptr, "null domain_weight_host");
   const int M = Bs + Bt;
   const int grid = train_stats_grid(M);
   const size_t need = ta3n_train_stats_workspace_bytes(M);
-  TA3N_REQUIRE(workspace && reinterpret_cast<uintptr_t>(workspace) % 16 == 0, "null or misaligned workspace");
+  TA3N_REQUIRE_WHO(workspace && reinterpret_cast<uintptr_t>(workspace) % 16 == 0, "null or misaligned workspace");
   if (workspace_bytes < need)
-    return fail(TA3N_ERR_WORKSPACE, "ta3n_train_stats_accumulate: workspace too small (%zu < %zu bytes)",
-                workspace_bytes, need);
+    return fail(TA3N_ERR_WORKSPACE, "%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
   TrainStatsArgs a;
-  a.pred_video = pred_video, a.labels = labels, a.pred_rel = pred_rel, a.pred_dom = pred_dom_video;
+  a.pred_video = pred_video, a.labels = labels, a.labels_t = labels_t, a.prec_sum = prec_sum;
+  a.pred_rel = pred_rel, a.pred_dom = pred_dom_video;
   a.pred_frame = pred_frame, a.pred2_s = pred2_s, a.pred2_t = pred2_t, a.loss = loss, a.valid_rows = valid_rows;
   a.class_weight = class_weight, a.accum = accum;
   a.dw[0] = domain_weight_host[0], a.dw[1] = domain_weight_host[1];
@@ -1281,6 +1331,30 @@ int ta3n_train_stats_accumulate(const float* pred_video, const long long* labels
   launch_kernel(train_stats_kernel, grid, kStatsThreads, 0, S(stream), a,
                 reinterpret_cast<TrainStatsPartial*>(workspace));
   return after_launch();
+}
+
+int ta3n_train_stats_accumulate(const float* pred_video, const long long* labels, const float* pred_rel,
+                                const float* pred_dom_video, const float* pred_frame, const float* pred2_s,
+                                const float* pred2_t, const float* loss, int Bs, int Bt, int T, int R, int C,
+                                int flags, const int* valid_rows, const float* class_weight,
+                                const float* domain_weight_host, int n_k, const int* k_host, ta3n_train_stats* accum,
+                                void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
+  return train_stats("ta3n_train_stats_accumulate", pred_video, labels, nullptr, pred_rel, pred_dom_video, pred_frame,
+                     pred2_s, pred2_t, loss, Bs, Bt, T, R, C, flags, valid_rows, class_weight, domain_weight_host, n_k,
+                     k_host, accum, nullptr, workspace, workspace_bytes, stream);
+}
+
+int ta3n_train_stats_accumulate_sv(const float* pred_video, const long long* labels, const long long* labels_t,
+                                   const float* pred_rel, const float* pred_dom_video, const float* pred_frame,
+                                   const float* loss, int Bs, int Bt, int T, int R, int C, int flags,
+                                   const int* valid_rows, const float* class_weight, const float* domain_weight_host,
+                                   int n_k, const int* k_host, ta3n_train_stats* accum, double* prec_sum,
+                                   void* workspace, size_t workspace_bytes, ta3n_stream_t stream) {
+  TA3N_REQUIRE(labels_t && prec_sum, "null target labels / prec_sum");
+  TA3N_REQUIRE(reinterpret_cast<uintptr_t>(prec_sum) % 8 == 0, "prec_sum must be 8-byte aligned");
+  return train_stats("ta3n_train_stats_accumulate_sv", pred_video, labels, labels_t, pred_rel, pred_dom_video,
+                     pred_frame, nullptr, nullptr, loss, Bs, Bt, T, R, C, flags, valid_rows, class_weight,
+                     domain_weight_host, n_k, k_host, accum, prec_sum, workspace, workspace_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -17,6 +17,8 @@ enum : int { STATS_REL = 1, STATS_VIDEO = 2, STATS_FRAME = 4, STATS_ENT = 8 };
 struct TrainStatsArgs {
   const float* pred_video;      // [M, C]; target rows: the logits the attentive entropy reads
   const long long* labels;      // [Bs]
+  const long long* labels_t;    // [Bt] or nullptr (use_target='Sv': the class CE and top-k cover the target rows too)
+  double* prec_sum;             // [n_k] with labels_t: sum over steps of the top-k percent * vs, else nullptr
   const float* pred_rel;        // [M, R, 2]
   const float* pred_dom;        // [M, 2]
   const float* pred_frame;      // [M * T, 2]
@@ -92,9 +94,10 @@ train_stats_kernel(const __grid_constant__ TrainStatsArgs a, TrainStatsPartial* 
   if (real) {
     const float* z = a.pred_video + (size_t)m * a.C;
     const RowStats rs = row_stats(z, a.C, lane);
-    if (!d) {
-      // class CE (criterion, main.py:446) and the rank of the label (accuracy, main.py:565-567)
-      const long long y = a.labels[m];
+    if (!d || a.labels_t) {
+      // class CE (criterion, main.py:446) and the rank of the label (accuracy, main.py:565-567); under Sv the target
+      // rows with their labels too (main.py:442-444)
+      const long long y = d ? a.labels_t[m - a.Bs] : a.labels[m];
       const bool in_range = y >= 0 && y < a.C;
       const float zy = in_range ? z[y] : 0.f;
       int gt = 0, tie_before = 0;
@@ -108,7 +111,7 @@ train_stats_kernel(const __grid_constant__ TrainStatsArgs a, TrainStatsPartial* 
       const double w = !in_range ? 1.0 : (a.class_weight ? (double)a.class_weight[y] : 1.0);
       t[P_CWCE] = in_range ? w * (double)(rs.mx + rs.lse - zy) : (double)NAN;
       t[P_CW] = w;
-      if (mcd) {                                    // main.py:447-448: the same criterion on the second classifier
+      if (mcd && !d) {                              // main.py:447-448: the same criterion on the second classifier
         const float* z2 = a.pred2_s + (size_t)m * a.C;
         const RowStats r2 = row_stats(z2, a.C, lane);
         t[P_C2WCE] = in_range ? w * (double)(r2.mx + r2.lse - z2[y]) : (double)NAN;
@@ -244,6 +247,8 @@ train_stats_kernel(const __grid_constant__ TrainStatsArgs a, TrainStatsPartial* 
   for (int q = 0; q < a.n_k; ++q) {                                         // top1 / top5                  :565-571
     acc->correct[q] += tot.correct[q];
     acc->correct_step[q] = tot.correct[q];
+    // Sv: accuracy() over the vs + vt labelled rows, folded with n = vs
+    if (a.prec_sum && tot.n_src > 0) a.prec_sum[q] += 100.0 * (double)tot.correct[q] / (double)tot.n_src * (double)vs;
   }
   acc->rows += tot.n_src;
   acc->rows_step = tot.n_src;

@@ -410,6 +410,9 @@ class DevicePairedSampler:
         self.rows = [torch.zeros(n, device=dev, dtype=torch.int32) for n in self.lengths]
         self.labels = torch.zeros(self.lengths[0], device=dev, dtype=torch.int64)
         self.state = torch.zeros(2, device=dev, dtype=torch.int32)      # {iteration, arrival counter}
+        # the target label list: only a step that trains on the target labels (use_target='Sv') asks for it
+        self.labels_t = None
+        self._perm_t = None
         self.n_iter = 0        # iterations of the current epoch (0 before the first start_epoch)
         self.issued = 0        # of which run() has consumed
 
@@ -421,9 +424,20 @@ class DevicePairedSampler:
         for d, bank in enumerate(self.banks):
             self.rows[d].copy_(torch.from_numpy(bank.order[perms[d]].astype(np.int32)))
         self.labels.copy_(torch.from_numpy(self.banks[0].labels[perms[0]]))
+        self._perm_t = perms[1]
+        if self.labels_t is not None:
+            self.labels_t.copy_(torch.from_numpy(self.banks[1].labels[perms[1]]))
         self.rewind()
         self.n_iter = n_iter
         return n_iter
+
+    def enable_target_labels(self) -> None:
+        """Keep the target label list on the device too, so that ``enqueue_gather`` can fill the target slot labels
+        (``TrainStep(use_target='Sv')``); the current epoch's list is uploaded at once.  Idempotent."""
+        if self.labels_t is None:
+            self.labels_t = torch.zeros(self.lengths[1], device=self.device, dtype=torch.int64)
+            if self._perm_t is not None:
+                self.labels_t.copy_(torch.from_numpy(self.banks[1].labels[self._perm_t]))
 
     def rewind(self) -> None:
         """Restart the current epoch at iteration 0 (current stream)."""
@@ -438,15 +452,26 @@ class DevicePairedSampler:
         self.issued += 1
 
     def enqueue_gather(self, xs: torch.Tensor, xt: torch.Tensor, labels: torch.Tensor, valid: torch.Tensor,
-                       stream: int) -> None:
+                       stream: int, labels_t: Optional[torch.Tensor] = None) -> None:
         """Fill one input slot (source / target features, source labels, {real source rows, real target rows})
-        with the current iteration's batch and advance the device iteration index: one launch."""
+        with the current iteration's batch and advance the device iteration index: one launch.  ``labels_t``: the
+        slot's target labels, filled too (``ta3n_gather_batch_labelled``; needs ``enable_target_labels()``)."""
         from . import _lib
         (bs, bt), (s, t) = self.batch, self.banks
         if (xs.shape[0], xt.shape[0]) != (bs, bt) or tuple(xs.shape[1:]) != self.row_shape or \
                 tuple(xt.shape[1:]) != self.row_shape:
             raise ValueError(f"slot {tuple(xs.shape)} + {tuple(xt.shape)} does not match the sampler's batches "
                              f"{bs} + {bt} of {self.row_shape}")
+        if labels_t is not None:
+            if self.labels_t is None:
+                raise ValueError("target slot labels need enable_target_labels()")
+            _lib.check(_lib.load().ta3n_gather_batch_labelled(
+                s.features.data_ptr(), s.features.shape[0], self.rows[0].data_ptr(), self.labels.data_ptr(),
+                self.lengths[0], bs, xs.data_ptr(), labels.data_ptr(),
+                t.features.data_ptr(), t.features.shape[0], self.rows[1].data_ptr(), self.labels_t.data_ptr(),
+                self.lengths[1], bt, xt.data_ptr(), labels_t.data_ptr(),
+                s.features.shape[1], valid.data_ptr(), self.state.data_ptr(), stream))
+            return
         _lib.check(_lib.load().ta3n_gather_batch(
             s.features.data_ptr(), s.features.shape[0], self.rows[0].data_ptr(), self.labels.data_ptr(),
             self.lengths[0], bs, xs.data_ptr(), labels.data_ptr(),

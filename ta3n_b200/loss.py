@@ -27,12 +27,24 @@ def dis_MCD(out1, out2):
 
 
 def ta3n_loss(outputs, label_source, gamma=0.003, place_adv=('Y', 'Y', 'Y'), use_attn='TransAttn',
-              add_loss_DA='attentive_entropy'):
-    """Loss of the shipped configuration (use_target='uSv', adv_DA='RevGrad'):
+              add_loss_DA='attentive_entropy', use_target='uSv', label_target=None):
+    """Loss of the shipped configuration (adv_DA='RevGrad'):
     main.py:446 (source CE) + main.py:508-538 (domain CE per level) + main.py:541-545 (target entropy; 0 without a
-    target row) or main.py:559-562 (attentive entropy)."""
+    target row) or main.py:559-562 (attentive entropy).
+    use_target: 'uSv' (default) as above; 'Sv' takes the class CE over cat(out_source, out_target) against
+    cat(label_source, label_target) (main.py:442-446), every other term unchanged; 'none' is the CE of the source rows
+    alone (main.py guards every DA term with use_target != 'none')."""
     (_, out_s, _, pd_s, _, _, out_t, _, pd_t, _) = outputs
-    loss = F.cross_entropy(out_s, label_source)
+    if use_target not in ('uSv', 'Sv', 'none'):
+        raise ValueError(f"use_target must be 'uSv', 'Sv' or 'none', got {use_target!r}")
+    if use_target == 'none':
+        return F.cross_entropy(out_s, label_source)
+    if use_target == 'Sv':
+        if label_target is None or tuple(label_target.shape) != (out_t.size(0),):
+            raise ValueError(f"use_target='Sv' needs label_target with one label per target row ({out_t.size(0)})")
+        loss = F.cross_entropy(torch.cat([out_s, out_t], 0), torch.cat([label_source, label_target], 0))
+    else:
+        loss = F.cross_entropy(out_s, label_source)
     per_level = []
     for lvl, flag in enumerate(place_adv):
         if flag != 'Y':

@@ -95,7 +95,9 @@ class TrainStats:
     """The meters of main.py's train() (main.py:311-320) over the steps since the last ``reset_stats()``: ``loss``,
     ``loss_c``, ``loss_a``, ``loss_e``, ``loss_s`` and, per k of ``topk``, the precision meter ``prec[k]`` (percent;
     ``top1`` / ``top5`` when those k are kept).  A meter whose term is switched off keeps count 0.  ``correct`` and
-    ``rows``: the epoch's top-k hits and real source rows; ``steps``: the steps folded in.  ``loss_d``: the
+    ``rows``: the epoch's top-k hits and real source rows -- under use_target='Sv' the hits and rows of the source AND
+    target rows, so correct / rows is not the top-k meter's average there (main.py weights each step's accuracy by its
+    source rows; read ``prec``); ``steps``: the steps folded in.  ``loss_d``: the
     discrepancy term without alpha (``losses_d``, main.py:504) under dis_DA 'DAN' / 'JAN', else empty."""
     loss: Meter
     loss_c: Meter
@@ -142,8 +144,9 @@ class TrainStatsSnapshot:
     """``TrainStep.stats_async()``: the accumulator copied to pinned host memory behind an event."""
 
     def __init__(self, host: torch.Tensor, event, topk: Tuple[int, ...], dis_host: Optional[torch.Tensor] = None,
-                 ent_host: Optional[torch.Tensor] = None):
+                 ent_host: Optional[torch.Tensor] = None, prec_host: Optional[torch.Tensor] = None):
         self._host, self._event, self._topk, self._dis_host, self._ent_host = host, event, topk, dis_host, ent_host
+        self._prec_host = prec_host
 
     def done(self) -> bool:
         return self._event.query()
@@ -156,7 +159,20 @@ class TrainStatsSnapshot:
             st.loss_d = dis_meter(self._dis_host.numpy())
         if self._ent_host is not None:
             st.loss_e = dis_meter(self._ent_host.numpy())
+        if self._prec_host is not None:
+            sv_prec(st, self._prec_host.numpy())
         return st
+
+
+def sv_prec(st: TrainStats, prec_sum) -> None:
+    """The top-k meters of ``ta3n_train_stats_accumulate_sv`` in place: accuracy() over the labelled source and target
+    rows (the hit counts of the accumulator), folded with n = the real source rows (main.py:565-571), whose sums are
+    ``prec_sum`` and whose count is loss_c's."""
+    n = st.loss_c.count
+    for q, k in enumerate(st.topk):
+        old = st.prec[k]
+        total = float(prec_sum[q])
+        st.prec[k] = Meter(val=old.val, avg=total / n if n else 0.0, sum=total, count=n)
 
 
 def dis_meter(words) -> Meter:
@@ -418,7 +434,8 @@ class TrainStep:
                  class_weight: Optional[torch.Tensor] = None, domain_weight: Sequence[float] = (1.0, 1.0),
                  allreduce: Optional[str] = None, mu: float = 0.0, sampler=None, stats: bool = False,
                  stats_topk: Sequence[int] = (1, 5), dis_DA: str = "none", alpha: float = 0.0,
-                 place_dis: Sequence[str] = ("Y", "Y", "N"), pretrain_source: bool = False):
+                 place_dis: Sequence[str] = ("Y", "Y", "N"), pretrain_source: bool = False,
+                 use_target: str = "uSv"):
         """mode: 'legacy' (default) = the per-operator sequence (25 launches in one CUDA graph; the only mode that
         supports use_attn_frame); 'phased' = the step program as 14 launches (ta3n_step_run_phased; default when class /
         domain weights or a scheduled beta are given).  class_weight / domain_weight: the weights of criterion /
@@ -481,7 +498,22 @@ class TrainStep:
         the TRN, the classifier(s), the relation discriminators under use_attn and the frame discriminator under frame
         attention; torch.optim skips the others, whose .grad is None).  Then the adaptation iteration above runs on the
         updated weights.  ``loss``, the meters and the gradients left in ``.grad`` are the adaptation pass's; Adam
-        counts two steps per iteration for P's parameters and one for the others, as torch.optim.Adam does."""
+        counts two steps per iteration for P's parameters and one for the others, as torch.optim.Adam does.
+
+        use_target: what the target domain is used for (main.py --use_target).  'uSv' (default): unsupervised
+        adaptation, the iteration above.  'Sv' (mode 'legacy', single rank; class / domain weights and a negative beta
+        are refused; ens_DA='MCD' raises NotImplementedError, as main.py:448 then fails): the class CE runs over the
+        real source AND target rows with the target labels (main.py:442-446; ``ta3n_loss_fwd_bwd_sv``), every DA term
+        as configured.  ``load`` / ``prefetch`` / ``__call__`` then need ``target_labels`` and a device sampler also
+        gathers them.  With stats=True, loss_c and top-k are main.py's: over the source and target rows, n = the real
+        source rows (``ta3n_train_stats_accumulate_sv``).  'none' (same refusals; a model with ens_DA='MCD' raises
+        ValueError, as main.py:74 never builds one): the source-only baseline.  The iteration is the source pass of
+        pretrain_source with the step's own dropout masks -- forward of the source rows, CE (main.py:446), backward,
+        clip and the optimizer over P; the other parameters' gradient slots stay zero and they get no update (two
+        such updates with pretrain_source, so Adam counts two steps for P).  beta, gamma, place_adv, add_loss_DA,
+        dis_DA and alpha are accepted and ignored, as main.py ignores them; target features passed to ``load`` are not
+        copied (a device sampler still gathers them: its one launch keeps the two domains' epoch positions paired).
+        With stats=True: loss, loss_c and top-k over the real source rows; loss_a / loss_e / loss_s keep count 0."""
         if optimizer is not None and not isinstance(optimizer, (SGDNesterov, Adam)):
             raise TypeError(f"optimizer must be SGDNesterov or Adam, got {type(optimizer).__name__}")
         if isinstance(optimizer, Adam):
@@ -511,6 +543,30 @@ class TrainStep:
             raise NotImplementedError("TrainStep covers frame_aggregation='trn-m', use_attn in ('TransAttn', 'none') and "
                                       "ens_DA in ('none', 'MCD'); train the other variants with model(...) + "
                                       "loss.backward()")
+        if use_target not in ("uSv", "Sv", "none"):
+            raise ValueError(f"use_target must be 'uSv', 'Sv' or 'none', got {use_target!r}")
+        self.use_target = use_target
+        if use_target != "uSv":
+            if ens == "MCD":
+                if use_target == "none":
+                    raise ValueError("use_target='none' with ens_DA='MCD': main.py:74 builds the source-only model "
+                                     "without MCD; build VideoModel(..., ens_DA='none')")
+                raise NotImplementedError("use_target='Sv' with ens_DA='MCD': main.py:448 applies the second "
+                                          "classifier's source logits to the source and target labels and fails")
+            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
+                raise NotImplementedError(f"use_target={use_target!r} runs in mode='legacy' only (the step program "
+                                          "has the unsupervised loss only)")
+            if class_weight is not None or any(float(b) < 0 for b in beta) or \
+                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
+                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
+                                          f"(mode='phased'), which does not cover use_target={use_target!r}")
+            if (dist.get_world_size(process_group) if dist.is_initialized() else 1) > 1:
+                # the target labels (Sv) would have to be sharded with the target rows
+                raise NotImplementedError(f"use_target={use_target!r} runs on a single rank")
+            mode = "legacy"
+            if use_target == "none":
+                # main.py guards every DA term with use_target != 'none' (:455, :508, :542, :548, :559)
+                place_adv, add_loss_DA, dis_DA, alpha = ("N", "N", "N"), "none", "none", 0.0
         self.add_fc = int(getattr(model, "add_fc", 1))
         if self.add_fc > 1:
             # the step program (phased) and what only it carries -- class / domain weights, the DANN beta schedule --
@@ -624,9 +680,9 @@ class TrainStep:
             raise ValueError("class_weight needs mode='phased'")
         self._overlap_requested = bool(overlap_allreduce)
         self.split = (self.world > 1) if overlap_allreduce is None else bool(overlap_allreduce)
-        if model.use_attn_frame != "none" or mode != "legacy" or self.mcd:
+        if model.use_attn_frame != "none" or mode != "legacy" or self.mcd or use_target == "none":
             # frame attention couples the TRN and frame-discriminator gradients; MCD's second pass adds to the early
-            # bucket after the first pass has finished it
+            # bucket after the first pass has finished it; use_target='none' runs the source pass, which has no split
             self.split = False
         # graph_collectives=True captures the two NCCL all-reduces INSIDE the step's graph.  It works and is
         # marginally faster (N=2: 0.371 vs 0.378 ms/step) but process-group teardown then hangs while the graphs
@@ -654,6 +710,7 @@ class TrainStep:
         # optimizer state (SURVEY 8f n2): momentum buffers (SGD) or the two moments and the step count (Adam),
         # device-resident learning rate, {norm, coef} stats
         self.opt = optimizer
+        self.active_mask = None
         self._opt_stepped = False           # SGD: an update has run or been loaded (torch's state is empty before)
         if optimizer is not None:
             if isinstance(optimizer, Adam):
@@ -696,6 +753,12 @@ class TrainStep:
                             for _ in range(self.n_slots)]
         self.active = 0
         self.xs, self.xt, self.labels, self.valid = self.slots[0]
+        # Sv: per slot, the target labels (padded rows keep what they held: the loss masks them out)
+        self.slot_labels_t = [torch.zeros(self.Bt, device=dev, dtype=torch.int64) for _ in range(self.n_slots)] \
+            if use_target == "Sv" else None
+        self.labels_t = self.slot_labels_t[0] if self.slot_labels_t else None
+        if sampler is not None and use_target == "Sv":
+            sampler.enable_target_labels()
         self.copy_stream = torch.cuda.Stream(device=dev) if double_buffer else None
         self.ready = [None] * self.n_slots          # event: slot filled
         self.consumed = [None] * self.n_slots       # event: last step that read the slot has finished
@@ -728,8 +791,12 @@ class TrainStep:
             add_fc=self.add_fc, drop_stack=self._stack_drops(seed, di))
         if self.mcd:
             self._init_mcd(seed, di, dv, offs)
-        if self.pretrain:
+        if self.pretrain or use_target == "none":
             self._init_pretrain(seed, di, dv, offs)
+        if use_target == "none":
+            # the iteration is the source pass with the step's own masks; its update covers P only
+            self.spec_src = self._source_spec(seed, di, dv)
+            self.active_mask = self.pretrain_mask if optimizer is not None else None
         self._init_stats(stats, stats_topk)
         self._init_dis(dis_DA, alpha, place_dis)
         if self.target_entropy and self.mcd and self.pred_video_t1 is None:
@@ -753,11 +820,9 @@ class TrainStep:
                 self._build_step(slot)
         if use_graph:
             for slot in range(self.n_slots):
-                self.active = slot
-                self.xs, self.xt, self.labels, self.valid = self.slots[slot]
+                self._activate(slot)
                 self.graphs[slot] = self._capture()
-            self.active = 0
-            self.xs, self.xt, self.labels, self.valid = self.slots[0]
+            self._activate(0)
         if sampler is not None:
             sampler.rewind()        # the capture's warm-up ran one gather
         if self.keep_stats:
@@ -848,6 +913,8 @@ class TrainStep:
         self.stats_stream = torch.cuda.Stream(device=self.device) if not self.split else None
         # the per-operator sequence's loss kernel has no domain weights (the step program applies them)
         self._stats_dw = (C.c_float * 2)(*(self.domain_weight if self.mode != "legacy" else (1.0, 1.0)))
+        # Sv: the fp64 sums of the top-k meters (ta3n_train_stats_accumulate_sv)
+        self.prec_sum = torch.zeros(4, device=self.device, dtype=torch.float64) if self.use_target == "Sv" else None
 
     def _enqueue_stats(self, lib, st, pred_video, pred_rel, pred_dom, pred_frame):
         """The meters of this step (after the loss launches; reads logits and the loss, writes the accumulator), on
@@ -858,9 +925,18 @@ class TrainStep:
             ev.record(torch.cuda.current_stream())
             self.stats_stream.wait_event(ev)
             st = self.stats_stream.cuda_stream
+        if self.use_target == "Sv":
+            check(lib.ta3n_train_stats_accumulate_sv(
+                _P(pred_video), _P(self.labels), _P(self.labels_t), _P(pred_rel), _P(pred_dom), _P(pred_frame),
+                _P(self.loss), self.Bs, self.Bt, self.T, self.R, self.C, self.flags, _P(self.valid),
+                _P(self.class_weight), self._stats_dw, len(self.stats_topk), self._stats_k, _P(self.stats_acc),
+                _P(self.prec_sum), _P(self.stats_ws), self.stats_ws.numel(), st))
+            return
+        # use_target='none': the source rows of the source pass, no domain term (Bt = 0, flags = 0)
+        bt = 0 if self.use_target == "none" else self.Bt
         check(lib.ta3n_train_stats_accumulate(
             _P(pred_video), _P(self.labels), _P(pred_rel), _P(pred_dom), _P(pred_frame), _P(p2s), _P(p2t),
-            _P(self.loss), self.Bs, self.Bt, self.T, self.R, self.C, self.flags, _P(self.valid),
+            _P(self.loss), self.Bs, bt, self.T, self.R, self.C, self.flags, _P(self.valid),
             _P(self.class_weight), self._stats_dw, len(self.stats_topk), self._stats_k, _P(self.stats_acc),
             _P(self.stats_ws), self.stats_ws.numel(), st))
 
@@ -880,6 +956,8 @@ class TrainStep:
             st.loss_d = dis_meter(self.dis_meter.cpu().numpy())
         if self.ent_meter is not None:
             st.loss_e = dis_meter(self.ent_meter.cpu().numpy())
+        if self.prec_sum is not None:
+            sv_prec(st, self.prec_sum.cpu().numpy())
         return st
 
     def stats_async(self) -> TrainStatsSnapshot:
@@ -896,9 +974,13 @@ class TrainStep:
         if self.ent_meter is not None:
             ent_host = torch.empty(3, dtype=torch.float64, pin_memory=True)
             ent_host.copy_(self.ent_meter, non_blocking=True)
+        prec_host = None
+        if self.prec_sum is not None:
+            prec_host = torch.empty(4, dtype=torch.float64, pin_memory=True)
+            prec_host.copy_(self.prec_sum, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
-        return TrainStatsSnapshot(host, ev, self.stats_topk, dis_host, ent_host)
+        return TrainStatsSnapshot(host, ev, self.stats_topk, dis_host, ent_host, prec_host)
 
     def reset_stats(self) -> None:
         """Start an epoch of meters (main.py builds fresh AverageMeters in every train() call): zeroes the accumulator
@@ -909,6 +991,8 @@ class TrainStep:
             self.dis_meter.zero_()
         if self.ent_meter is not None:
             self.ent_meter.zero_()
+        if self.prec_sum is not None:
+            self.prec_sum.zero_()
 
     def _stack_drops(self, seed, di):
         """dropout_i of the stacked shared layers: one seed per layer (``stack_seed``), the step counter as key."""
@@ -989,13 +1073,7 @@ class TrainStep:
         Bs, C, R = self.Bs, self.C, self.R
         s = (seed ^ _PRETRAIN_KEY) & (2 ** 63 - 1)
         self.pretrain_seeds = (s, s ^ 0x9E3779B9)      # (drop_i, drop_v), keyed by the same step counter
-        # CE on the class logits only: no video discriminator, and the frame discriminator only under frame attention
-        self.spec_pre = TF.PathSpec(
-            num_segments=self.T, beta=self.spec.beta, mu=0.0, reverse=False, use_attn=self.spec.use_attn,
-            use_attn_frame=self.spec.use_attn_frame, classify_only=True,
-            drop_i=TF.DropSpec(p=di, seed=s, step=self.step_counter) if di > 0 else TF.DropSpec(),
-            drop_v=TF.DropSpec(p=dv, seed=s ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec(),
-            add_fc=self.add_fc, drop_stack=self._stack_drops(s, di))
+        self.spec_pre = self._source_spec(s, di, dv)
         self.bufs_pre = TF.Buffers(dev, persistent=True)
         self.x_none = torch.zeros(0, self.T, self.D, **f32)            # the pass has no target half
         self.loss_pre = torch.zeros(1, **f32)
@@ -1031,15 +1109,31 @@ class TrainStep:
         if isinstance(self.opt, Adam):
             self.adam_step_pre = torch.zeros(1, device=dev, dtype=torch.int64)
 
-    def _enqueue_pretrain(self, lib, st, optimizer):
+    def _source_spec(self, s, di, dv):
+        """The source-only pass with dropout seeds (s, s ^ 0x9E3779B9) keyed by the step counter: CE on the class
+        logits only, so no video discriminator, and the frame discriminator only under frame attention."""
+        return TF.PathSpec(
+            num_segments=self.T, beta=self.spec.beta, mu=0.0, reverse=False, use_attn=self.spec.use_attn,
+            use_attn_frame=self.spec.use_attn_frame, classify_only=True,
+            drop_i=TF.DropSpec(p=di, seed=s, step=self.step_counter) if di > 0 else TF.DropSpec(),
+            drop_v=TF.DropSpec(p=dv, seed=s ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec(),
+            add_fc=self.add_fc, drop_stack=self._stack_drops(s, di))
+
+    def _enqueue_pretrain(self, lib, st, optimizer, spec=None, loss=None, after_loss=None):
         """The pre-training update (main.py:388-414): the source rows' forward, CE (+ CE of the second classifier),
-        the backward into the gradient bucket, the slots outside P zeroed, then clip + the optimizer over P."""
+        the backward into the gradient bucket, the slots outside P zeroed, then clip + the optimizer over P.
+        use_target='none' runs its iteration as this pass with ``spec`` (the step's masks) and ``loss`` (the step's
+        loss); ``after_loss(outputs)`` is called once the loss is written (the meters' launch)."""
         Bs, C = self.Bs, self.C
-        saved, outputs, dims = TF.path_forward(self.spec_pre, self.xs, self.x_none, self.params[:self.n_path],
+        spec = self.spec_pre if spec is None else spec
+        loss = self.loss_pre if loss is None else loss
+        saved, outputs, dims = TF.path_forward(spec, self.xs, self.x_none, self.params[:self.n_path],
                                                self.bufs_pre, batch_gemms=True)
-        self.loss_pre.zero_()
-        check(lib.ta3n_ce_loss_fwd_bwd(_P(outputs[5]), _P(self.labels), Bs, C, _P(self.valid), _P(self.loss_pre),
+        loss.zero_()
+        check(lib.ta3n_ce_loss_fwd_bwd(_P(outputs[5]), _P(self.labels), Bs, C, _P(self.valid), _P(loss),
                                        _P(self.g_video_pre), st))
+        if after_loss is not None:
+            after_loss(outputs)
         gin = {"pred_video": self.g_video_pre}
         check(lib.ta3n_wgrad_defer_begin())
         if self.mcd:
@@ -1052,7 +1146,7 @@ class TrainStep:
             self._enqueue_head2_bwd(lib, st, self.bufs_pre, saved["dropped"], Bs, self.g_video2_pre, d_dropped,
                                     self.grad_views)
             gin["dropped"] = d_dropped
-        TF.path_backward(self.spec_pre, dims, self.xs, self.x_none, self.params[:self.n_path], saved, gin,
+        TF.path_backward(spec, dims, self.xs, self.x_none, self.params[:self.n_path], saved, gin,
                          self.grad_views[:self.n_path], self.bufs_pre)
         ws = self.bufs_pre.workspace("wgrad", lib.ta3n_wgrad_defer_workspace_bytes())
         check(lib.ta3n_wgrad_defer_flush(_P(ws), ws.numel(), st))
@@ -1219,7 +1313,9 @@ class TrainStep:
     def _optimizer_launches(self) -> int:
         """Launches of the optimizer updates of one iteration (those of the pre-training update included)."""
         calls = 1
-        if self.pretrain:
+        if self.use_target == "none":
+            calls = 2 if self.pretrain else 1          # P only, once per source pass
+        elif self.pretrain:
             calls = 2 + (1 if isinstance(self.opt, Adam) and self.pretrain_rest is not None else 0)
         return calls * (2 if self.opt.clip_gradient is not None else 1)
 
@@ -1259,8 +1355,12 @@ class TrainStep:
         if self.opt is None:
             raise ValueError("optimizer_state_dict needs TrainStep(optimizer=...)")
         if isinstance(self.opt, Adam):
-            # with pretrain_source P's count is 2k after k iterations (the rest of the set may be empty)
-            step = int(self.adam_step_pre.item()) // 2 if self.pretrain else int(self.adam_step.item())
+            # with pretrain_source P's count is 2k after k iterations (the rest of the set may be empty); under
+            # use_target='none' P is the whole set and its count is k (2k with pretrain_source)
+            if self.use_target == "none":
+                step = int(self.adam_step_pre.item()) // (2 if self.pretrain else 1)
+            else:
+                step = int(self.adam_step_pre.item()) // 2 if self.pretrain else int(self.adam_step.item())
         else:
             step = int(self._opt_stepped)
         return optimizer_state_to_torch(self.model, self.opt, self._flat_state(), self.active_mask, step,
@@ -1283,6 +1383,8 @@ class TrainStep:
             self.adam_step.fill_(step)
             if self.pretrain:
                 self.adam_step_pre.fill_(2 * step)
+            elif self.use_target == "none":
+                self.adam_step_pre.fill_(step)
         self._opt_stepped = step > 0
 
     def state_dict(self) -> dict:
@@ -1323,7 +1425,8 @@ class TrainStep:
 
     def _enqueue_body(self, lib, st, at_split, optimizer):
         if self.sampler is not None:
-            self.sampler.enqueue_gather(self.xs, self.xt, self.labels, self.valid, st)     # this iteration's batch
+            self.sampler.enqueue_gather(self.xs, self.xt, self.labels, self.valid, st,     # this iteration's batch
+                                        labels_t=self.labels_t)
         if self.mode != "legacy":
             check(lib.ta3n_step_run_phased(C.byref(self.step_descs[self.active][0]), st))
             if self.keep_stats:
@@ -1338,6 +1441,9 @@ class TrainStep:
         check(lib.ta3n_counter_inc(_P(self.step_counter), st))          # fresh dropout masks per step
         if self.pretrain:
             self._enqueue_pretrain(lib, st, optimizer and self.opt is not None)
+        if self.use_target == "none":
+            self._enqueue_source_only(lib, st, optimizer and self.opt is not None)
+            return
         saved, outputs, dims = TF.path_forward(self.spec, self.xs, self.xt, self.params[:self.n_path], self.bufs,
                                                batch_gemms=True)
         self.outputs = outputs
@@ -1350,10 +1456,17 @@ class TrainStep:
             if self.pred_video_t1 is not None:
                 self.pred_video_t1.copy_(pred_video[self.Bs:])      # pass 2 writes its target logits over these
             saved2, dims2 = self._enqueue_mcd_pass2_forward(lib, st)
-        check(lib.ta3n_loss_fwd_bwd(_P(pred_video), _P(self.labels), _P(pred_rel), _P(pred_dom), _P(pred_frame),
-                                    self.Bs, self.Bt, self.T, self.R, self.C, self.gamma, self.flags,
-                                    _P(self.valid), _P(self.loss), _P(self.g_video), _P(self.g_rel), _P(self.g_dom),
-                                    _P(self.g_frame), _P(self.loss_ws), self.loss_ws.numel(), st))
+        if self.use_target == "Sv":
+            check(lib.ta3n_loss_fwd_bwd_sv(
+                _P(pred_video), _P(self.labels), _P(self.labels_t), _P(pred_rel), _P(pred_dom), _P(pred_frame),
+                self.Bs, self.Bt, self.T, self.R, self.C, self.gamma, self.flags, _P(self.valid), _P(self.loss),
+                _P(self.g_video), _P(self.g_rel), _P(self.g_dom), _P(self.g_frame), _P(self.loss_ws),
+                self.loss_ws.numel(), st))
+        else:
+            check(lib.ta3n_loss_fwd_bwd(_P(pred_video), _P(self.labels), _P(pred_rel), _P(pred_dom), _P(pred_frame),
+                                        self.Bs, self.Bt, self.T, self.R, self.C, self.gamma, self.flags,
+                                        _P(self.valid), _P(self.loss), _P(self.g_video), _P(self.g_rel),
+                                        _P(self.g_dom), _P(self.g_frame), _P(self.loss_ws), self.loss_ws.numel(), st))
         if self.mcd:
             check(lib.ta3n_ce_loss_fwd_bwd(_P(self.pred2_s), _P(self.labels), self.Bs, self.C, _P(self.valid),
                                            _P(self.loss), _P(self.g_video2), st))
@@ -1436,6 +1549,17 @@ class TrainStep:
             self._enqueue_optimizer()
         self._join_stats()
 
+    def _enqueue_source_only(self, lib, st, optimizer):
+        """use_target='none' (main.py:418-583 with every DA term off): the source pass with the step's dropout masks
+        and loss, the meters on its source logits, its update over P."""
+        def stats(outputs):
+            self.outputs = outputs
+            if self.keep_stats:
+                # flags == 0: no domain logits are read (the pass makes none); the entry wants addresses all the same
+                self._enqueue_stats(lib, st, outputs[5], self.g_rel, self.g_dom, self.g_frame)
+        self._enqueue_pretrain(lib, st, optimizer, self.spec_src, self.loss, stats)
+        self._join_stats()
+
     def _enqueue_with_collectives(self, optimizer=False):
         """The step with both gradient all-reduces issued in place (early bucket as soon as it is complete)."""
         pending = []
@@ -1497,19 +1621,26 @@ class TrainStep:
         return (ga, gb)
 
     # -- public API ------------------------------------------------------------------------------------
-    def _fill(self, slot, source, target, labels):
+    def _fill(self, slot, source, target, labels, target_labels=None):
         """Copy a paired mini-batch into input slot `slot` on the current stream.  Fewer than (Bs, Bt) rows --
         the last batch of an epoch -- are padded the way main.py:354-372 does and masked out of every loss term
         the way main.py:421-422 does (the rows are simply left as they were: rows are independent and the
-        padded ones receive zero gradient)."""
+        padded ones receive zero gradient).  use_target='Sv' needs ``target_labels``, one per target row; under
+        'none' the target rows feed nothing and are not copied."""
         xs, xt, lab, valid = self.slots[slot]
         ns, nt = int(source.shape[0]), int(target.shape[0])
         if not (1 <= ns <= self.Bs and 0 <= nt <= self.Bt) or labels.shape[0] != ns:
             raise ValueError(f"batch of {ns}+{nt} videos / {labels.shape[0]} labels does not fit TrainStep({self.Bs}, {self.Bt})")
+        if self.use_target == "Sv" and (target_labels is None or tuple(target_labels.shape) != (nt,)):
+            got = None if target_labels is None else tuple(target_labels.shape)
+            raise ValueError(f"use_target='Sv' needs target_labels of shape ({nt},) for the {nt} target videos, "
+                             f"got {got}")
         xs[:ns].copy_(source.reshape((ns,) + tuple(xs.shape[1:])), non_blocking=True)
-        if nt:
+        if nt and self.use_target != "none":
             xt[:nt].copy_(target.reshape((nt,) + tuple(xt.shape[1:])), non_blocking=True)
         lab[:ns].copy_(labels, non_blocking=True)
+        if self.use_target == "Sv" and nt:
+            self.slot_labels_t[slot][:nt].copy_(target_labels, non_blocking=True)
         host = self._valid_host[slot]
         if (int(host[0]), int(host[1])) != (ns, nt):
             # the pinned pair must not change while an earlier async copy of it may be pending; the batch size
@@ -1518,16 +1649,17 @@ class TrainStep:
             host[0], host[1] = ns, nt
             valid.copy_(host, non_blocking=True)
 
-    def load(self, source, target, labels):
-        """Copy one paired mini-batch (host or device tensors) into the ACTIVE input slot (compute stream)."""
+    def load(self, source, target, labels, target_labels=None):
+        """Copy one paired mini-batch (host or device tensors) into the ACTIVE input slot (compute stream).
+        ``target_labels``: the target rows' labels, needed under use_target='Sv' and ignored otherwise."""
         self._no_sampler("load")
-        self._fill(self.active, source, target, labels)
+        self._fill(self.active, source, target, labels, target_labels)
 
     def _no_sampler(self, what):
         if self.sampler is not None:
             raise RuntimeError(f"{what}() with a device sampler attached: run() gathers every batch itself")
 
-    def prefetch(self, source, target, labels):
+    def prefetch(self, source, target, labels, target_labels=None):
         """double_buffer=True: copy the NEXT mini-batch into the inactive slot on the copy stream, overlapping
         the step that is running; call ``swap()`` before the ``run()`` that should consume it."""
         self._no_sampler("prefetch")
@@ -1537,15 +1669,20 @@ class TrainStep:
         with torch.cuda.stream(self.copy_stream):
             if self.consumed[nxt] is not None:
                 self.copy_stream.wait_event(self.consumed[nxt])      # do not overwrite inputs still being read
-            self._fill(nxt, source, target, labels)
+            self._fill(nxt, source, target, labels, target_labels)
             ev = torch.cuda.Event()
             ev.record(self.copy_stream)
         self.ready[nxt] = ev
 
+    def _activate(self, slot):
+        self.active = slot
+        self.xs, self.xt, self.labels, self.valid = self.slots[slot]
+        if self.slot_labels_t is not None:
+            self.labels_t = self.slot_labels_t[slot]
+
     def swap(self):
         """Make the prefetched slot the active one (the compute stream waits for its copies)."""
-        self.active = 1 - self.active
-        self.xs, self.xt, self.labels, self.valid = self.slots[self.active]
+        self._activate(1 - self.active)
         if self.ready[self.active] is not None:
             torch.cuda.current_stream().wait_event(self.ready[self.active])
             self.ready[self.active] = None
@@ -1590,7 +1727,7 @@ class TrainStep:
         self.install_grads()
         return self.loss
 
-    def __call__(self, source, target, labels):
+    def __call__(self, source, target, labels, target_labels=None):
         self._no_sampler("__call__")
-        self.load(source, target, labels)
+        self.load(source, target, labels, target_labels)
         return self.run()
