@@ -4,7 +4,9 @@ loss.py:8-12) as one CUDA loss launch in the captured step.
 CPU: the oracle (oracle/target_entropy_oracle.py) against the reference's iteration (tests/golden/
 target_entropy_golden.npz, and the live reference where it is present), the options TrainStep refuses, the C ABI's
 argument checks.
-GPU: one step against the fp64 oracle on every engine (dropout off and on, MCD with mu 0 and 0.7, with DAN, short batches), a batch
+GPU: the entry alone against fp64 at fp32 grade (rows past the warps' first pass, classes past the lanes' first trip,
+clamped / absent valid_rows, underflowing and uniform rows, accumulation over launches); one step against the fp64
+oracle on every engine (dropout off and on, MCD with mu 0 and 0.7, with DAN, short batches), a batch
 with no target row against the step without the term, three SGD steps against the stock autograd loop, bit-identical
 reruns / eager vs graph / resume, the meters, and the launches the term adds.
 """
@@ -198,6 +200,92 @@ def engine(request):
     ta3n_b200.set_gemm_engine(request.param)
     yield request.param
     ta3n_b200.set_gemm_engine("tf32x3")
+
+
+def _entropy_logits(rows, C, seed):
+    """randn * 3, with (where the rows exist) a large-spread row whose q underflows for half the classes and a
+    uniform row (H = log C exactly, zero gradient)."""
+    g = torch.Generator().manual_seed(seed)
+    z = torch.randn(rows, C, generator=g) * 3
+    if rows > 1:
+        z[rows // 2] = torch.where(torch.rand(C, generator=g) < 0.5, -80.0, 80.0) + torch.randn(C, generator=g)
+    if rows > 2:
+        z[rows - 1] = 2.5
+    return z
+
+
+def _entropy_ref(dt, z, vt, gamma, L0, G0, calls):
+    """``calls`` launches from loss L0 and gradient G0: L0 + calls * gamma * term, G0 + calls * its gradient."""
+    from tests.test_rowops_fp32 import _leaf
+    p = _leaf(z, dt)
+    term = teo.target_entropy(p[:vt])
+    g = torch.autograd.grad(gamma * term, p)[0] if vt > 0 else torch.zeros_like(p)
+    return dict(term=term.detach(), loss=torch.tensor(L0, dtype=dt) + calls * gamma * term.detach(),
+                g=G0.to(dt) + calls * g)
+
+
+@gpu
+@pytest.mark.parametrize("C", [1, 7, 30, 32, 33, 1000])
+@pytest.mark.parametrize("rows", [1, 31, 32, 33, 1024, 1500])
+def test_entropy_entry_matches_fp64(rows, C):
+    """ta3n_target_entropy_fwd_bwd alone against fp64 (test_rowops_fp32's rule, per row): rows past the 32 warps'
+    first pass, classes past the lanes' first trip, valid_rows 0 / 1 / rows - 1 / rows / more than rows (clamped) and
+    absent.  The loss, the gradient and the meter accumulate over two launches; padded rows keep their values bit for
+    bit; a second run on fresh buffers gives the same bits."""
+    from ta3n_b200._lib import check as lib_check
+    from tests.test_rowops_fp32 import Buf, _guards, _lib, _ref, _st, check
+    _, lib = _lib()
+    gamma, L0, M0 = 0.7, 0.625, (3.5, -1.0, 11.0)
+    z = _entropy_logits(rows, C, rows * 1009 + C)
+    G0 = torch.randn(rows, C, generator=torch.Generator().manual_seed(C)) * 1e-3
+    H = teo.target_entropy(z[rows - 1:].double()).item() if rows > 2 else None
+    if H is not None:
+        assert abs(H - np.log(C)) <= 1e-12 * max(1.0, np.log(C))
+    for valid in sorted({0, 1, rows - 1, rows, rows + 5}) + [None]:
+        vt = rows if valid is None else min(valid, rows)
+        runs = []
+        for _ in range(2):
+            pb = Buf(rows, C, init=z.to(_dev()))
+            loss = Buf(1, init=torch.full((1,), L0, device=_dev()))
+            gp = Buf(rows, C, init=G0.to(_dev()))
+            meter = torch.tensor(M0, device=_dev(), dtype=torch.float64)
+            vr = None if valid is None else torch.tensor([17, valid], dtype=torch.int32, device=_dev())
+            lib_check(lib.ta3n_target_entropy_fwd_bwd(pb.p, rows, C, gamma, None if vr is None else vr.data_ptr(),
+                                                      loss.p, gp.p, meter.data_ptr(), _st()))
+            torch.cuda.synchronize()
+            runs.append((loss.cpu().clone(), gp.cpu().clone(), meter.cpu().clone()))
+        assert all(torch.equal(a, b) for a, b in zip(*runs)), f"rows={rows} C={C} valid={valid}: reruns differ"
+        what = f"rows={rows} C={C} valid={valid}"
+        r64, r32 = _ref(_entropy_ref, z, vt, gamma, L0, G0, 1)
+        q64 = torch.softmax(z.double(), 1)
+        lq64 = torch.log_softmax(z.double(), 1)
+        H64 = -(q64 * lq64).sum(1, keepdim=True)
+        # the summands behind each gradient element: its start value and gamma/n * q (|log q| + H)
+        scale = G0.double().abs() + gamma / max(vt, 1) * q64 * (lq64.abs() + H64)
+        check(f"{what} term", runs[0][2][1], r64["term"], r32["term"], scale=torch.tensor(max(np.log(C), 1.0)))
+        check(f"{what} loss", runs[0][0][0], r64["loss"], r32["loss"], scale=torch.tensor(L0 + gamma * np.log(C)))
+        check(f"{what} g_pred", runs[0][1], r64["g"], r32["g"], dims=(0,), scale=scale)
+        assert torch.equal(runs[0][1][vt:], G0[vt:]), f"{what}: a padded row's gradient changed"
+        if C == 1:
+            assert torch.equal(runs[0][1], G0) and runs[0][2][1].item() == 0.0
+        if vt == 0:
+            assert runs[0][0][0].item() == L0 and runs[0][2][1].item() == 0.0, f"{what}: no real row must add nothing"
+        term = runs[0][2][1].item()
+        assert runs[0][2][0].item() == M0[0] + term * vt and runs[0][2][2].item() == M0[2] + vt
+        # a second launch on the same buffers: everything accumulates, the last value is the same bits
+        vr = None if valid is None else torch.tensor([17, valid], dtype=torch.int32, device=_dev())
+        lib_check(lib.ta3n_target_entropy_fwd_bwd(pb.p, rows, C, gamma, None if vr is None else vr.data_ptr(), loss.p,
+                                                  gp.p, meter.data_ptr(), _st()))
+        torch.cuda.synchronize()
+        r64, r32 = _ref(_entropy_ref, z, vt, gamma, L0, G0, 2)
+        check(f"{what} loss x2", loss.t[0], r64["loss"], r32["loss"], scale=torch.tensor(L0 + 2 * gamma * np.log(C)))
+        check(f"{what} g_pred x2", gp.t, r64["g"], r32["g"], dims=(0,), scale=2 * scale)
+        m = meter.cpu()
+        assert m[1].item() == term and m[2].item() == M0[2] + 2 * vt
+        assert m[0].item() == (M0[0] + term * vt) + term * vt
+        assert torch.equal(gp.cpu()[vt:], G0[vt:])
+        _guards(pb, loss, gp)
+        assert torch.equal(pb.cpu(), z), "pred was written"
 
 
 @gpu

@@ -2,7 +2,8 @@
 
 CPU: the options TrainStep refuses with either value, the autograd loss (``loss.ta3n_loss(use_target=...)``) against
 main.py:442-446's composition, and the argument checks of the three new C entries.
-GPU: the Sv loss entry and the Sv meters entry against fp64 restatements; the labelled gather against the plain one;
+GPU: the Sv loss entry and the Sv meters entry against fp64 restatements, also at cfg5's 1024 rows (the meters' 128
+CTA partials); the labelled gather against the plain one;
 TrainStep iterations against the stock autograd loop with torch.optim (fp32 engine); bit-identical eager / graph /
 reruns / resume, device sampler and double buffering; 'uSv' equal to the default; the launches of 'none' and the
 parameters it leaves alone; the meters.
@@ -10,6 +11,7 @@ parameters it leaves alone; the meters.
 import copy
 import ctypes as C
 
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -249,6 +251,33 @@ def test_sv_loss_entry_matches_fp64(C, valid):
 
 
 @gpu
+@pytest.mark.parametrize("C", [30, 1000])
+@pytest.mark.parametrize("valid", [(512, 512), (500, 311)])
+def test_sv_loss_entry_at_full_size(C, valid):
+    """The Sv loss entry at cfg5's M = 1024 rows (Bs = Bt = 512), where its grid-stride loops make several trips:
+    the loss and every gradient against fp64, per row of the class logits' gradient too, padded rows zero."""
+    from ta3n_b200 import _lib
+    lib = _lib.load()
+    Bs, Bt, T, R = 512, 512, 5, 4
+    vs, vt = valid
+    pv, rel, dom, frame, ls, lt = _loss_inputs(Bs, Bt, T, R, C, seed=C)
+    loss, g = _loss_call(lib, "sv", pv, rel, dom, frame, ls, lt, Bs, Bt, T, R, C, 15, 0.3, valid)
+    want, wg = _loss_fp64(pv, rel, dom, frame, ls, lt, Bs, vs, vt, T, R, 15, 0.3)
+    assert abs(loss.double().item() - want.item()) <= 2e-6 * abs(want.item()) + 1e-6
+    pad = torch.ones(Bs + Bt, dtype=torch.bool)
+    pad[:vs] = False
+    pad[Bs:Bs + vt] = False
+    for got, ref, name in zip(g, wg, ("pred_video", "pred_rel", "pred_dom", "pred_frame")):
+        rows = got.view(Bs + Bt, -1)
+        assert torch.all(rows[pad] == 0), name
+        real, got_real = ref.view(Bs + Bt, -1)[~pad], rows[~pad].double()
+        assert_close(got_real, real, 2e-5, name, noise=1e-9)
+        err, den = (got_real - real).norm(dim=1), real.norm(dim=1)
+        bad = err > 2e-5 * den + 1e-9
+        assert not bool(bad.any()), f"{name}: row {int(torch.nonzero(bad)[0, 0])} off"
+
+
+@gpu
 def test_sv_loss_entry_equals_the_plain_entry_without_target_rows_and_handles_nan():
     """With no real target row the Sv entry is the plain entry, bit for bit; a NaN target logit makes the loss NaN and
     leaves the other rows' gradients finite."""
@@ -310,6 +339,54 @@ def test_sv_meters_entry_over_an_epoch():
         assert st.top1.count == 36 and st.top1.avg == pytest.approx(m1.avg, rel=1e-12)
         assert st.top5.avg == pytest.approx(m5.avg, rel=1e-12)
         assert st.top1.val == pytest.approx(m1.val, rel=1e-12)
+        runs.append((acc.cpu(), prec.cpu()))
+    assert torch.equal(runs[0][0], runs[1][0]) and torch.equal(runs[0][1], runs[1][1])
+
+
+@gpu
+@pytest.mark.parametrize("C", [5, 30, 101])
+def test_sv_meters_entry_at_full_size(C):
+    """The Sv meters at M = 1024 rows: 128 CTAs whose partials the last one to arrive folds.  An epoch of four
+    batches with a short last one against the oracle's fold (use_target_oracle.fold, train_stats_oracle.label_rank's
+    tie rule), and a second run of the epoch bit-identical to the first."""
+    from oracle import train_stats_oracle as tso
+    from oracle import use_target_oracle as uto
+    from ta3n_b200 import _lib
+    from ta3n_b200.train import _STATS_WORDS, parse_train_stats, sv_prec
+    lib = _lib.load()
+    d = _dev()
+    Bs, Bt, T, R = 512, 512, 5, 4
+    batches = [(512, 512), (512, 512), (512, 512), (300, 211)]
+    ws = torch.zeros(lib.ta3n_train_stats_workspace_bytes(Bs + Bt), device=d, dtype=torch.uint8)
+    runs = []
+    for _ in range(2):
+        acc = torch.zeros(_STATS_WORDS, device=d, dtype=torch.int64)
+        prec = torch.zeros(4, device=d, dtype=torch.float64)
+        steps = []
+        for i, (vs, vt) in enumerate(batches):
+            pv, rel, dom, frame, ls, lt = _loss_inputs(Bs, Bt, T, R, C, seed=40 + i)
+            ins = [t.to(d).contiguous() for t in (pv, rel, dom, frame, ls, lt)]
+            loss = torch.tensor([1.5 + i], device=d)
+            _stats_call(lib, acc, prec, ws, *ins, loss, Bs, Bt, T, R, C, 15, (vs, vt), (1, 5))
+            z = torch.cat([pv[:vs], pv[Bs:Bs + vt]]).double().numpy()
+            y = torch.cat([ls[:vs], lt[:vt]]).numpy()
+            rank = tso.label_rank(z, y)
+            steps.append({"loss": None, "loss_c": (float(tso._weighted_ce(z, y, None, np.float64)), vs),
+                          "loss_a": None, "loss_e": None, "loss_s": None,
+                          "correct": (int((rank < 1).sum()), int((rank < 5).sum())), "rows": vs + vt, "n": vs})
+        torch.cuda.synchronize()
+        want = uto.fold(steps)
+        st = parse_train_stats(acc.cpu().numpy(), (1, 5))
+        sv_prec(st, prec.cpu().numpy())
+        assert st.loss_c.count == want["loss_c"].count == 1836
+        assert st.loss_c.avg == pytest.approx(want["loss_c"].avg, rel=1e-6)
+        assert st.loss_c.val == pytest.approx(want["loss_c"].val, rel=1e-6)
+        for k in ("top1", "top5"):
+            got = getattr(st, k)
+            assert got.count == want[k].count and got.avg == pytest.approx(want[k].avg, rel=1e-12), k
+            assert got.val == pytest.approx(want[k].val, rel=1e-12), k
+        if C == 5:
+            assert st.top5.avg == 100.0
         runs.append((acc.cpu(), prec.cpu()))
     assert torch.equal(runs[0][0], runs[1][0]) and torch.equal(runs[0][1], runs[1][1])
 
