@@ -202,28 +202,53 @@ class PathSpec:
 #   rel-disc W1_i | b1_i | W2_i | b2_i (each R long) | classifier W,b | video-disc W1,b1,W2,b2
 #   [ | attn_layer W1,b1,w2,b2  -- only with PathSpec.general_attn ]
 #   [ | shared_2 W,b [ | shared_3 W,b ]  -- the stacked shared layers of add_fc 2 and 3 ]
+#   [ | classifier_2 W,b  -- ens_DA='MCD': TrainStep's flat buffers append the second classifier ]
+# frame_aggregation='avgpool' has the same order without the TRN and the relation discriminators, i.e. R = 0.
+@dataclass(frozen=True)
+class ParamLayout:
+    """Index groups of the parameter list above (``param_layout``)."""
+    shared: range
+    frame_disc: range
+    trn_w: range
+    trn_b: range
+    rel_disc: range             # W1_i | b1_i | W2_i | b2_i, each R long
+    classifier: range
+    video_disc: range
+    attn_layer: range           # empty without general attention
+    stack: range                # empty at add_fc=1
+    head2: range                # empty without MCD
+
+    @property
+    def n_core(self) -> int:
+        """The tensors the operator takes at add_fc=1."""
+        return self.stack.start
+
+
+def param_layout(R: int, general_attn: bool = False, add_fc: int = 1, mcd: bool = False) -> ParamLayout:
+    """The index groups of the path's parameter list for R = T - 1 relation scales (0 for avgpool)."""
+    sizes = (2, 4, R, R, 4 * R, 2, 4, 4 if general_attn else 0, 2 * (add_fc - 1), 2 if mcd else 0)
+    ends = list(itertools.accumulate(sizes, initial=0))
+    return ParamLayout(*(range(lo, hi) for lo, hi in zip(ends, ends[1:])))
+
+
 def _attn_layer_params(params, R, add_fc=1):
     """The four tensors of the 'general' attention layer (models.py:320-325), behind the core ones."""
-    n = 6 + 6 * R + 6
-    if len(params) != n + 4 + 2 * (add_fc - 1):
-        raise _lib.Ta3nError(f"general attention at add_fc={add_fc} expects {n + 4 + 2 * (add_fc - 1)} parameter "
+    lay = param_layout(R, True, add_fc)
+    if len(params) != lay.stack.stop:
+        raise _lib.Ta3nError(f"general attention at add_fc={add_fc} expects {lay.stack.stop} parameter "
                              f"tensors, got {len(params)}")
-    return params[n:n + 4]
+    return [params[i] for i in lay.attn_layer]
 
 
-def _stack_params(params, n_core, add_fc):
-    """[(W_2, b_2), (W_3, b_3)][:add_fc - 1]: the stacked shared layers' tensors, appended behind the ``n_core`` tensors
-    the operator takes at add_fc=1."""
+def _stack_params(params, R, add_fc, general_attn=False):
+    """[(W_2, b_2), (W_3, b_3)][:add_fc - 1]: the stacked shared layers' tensors, appended behind the tensors the
+    operator takes at add_fc=1."""
     if not 1 <= add_fc <= 3:
         raise _lib.Ta3nError(f"add_fc must be 1, 2 or 3 (models.py:141-153), got {add_fc}")
-    n = n_core + 2 * (add_fc - 1)
-    if len(params) != n:
-        raise _lib.Ta3nError(f"add_fc={add_fc} expects {n} parameter tensors, got {len(params)}")
-    return [(params[i], params[i + 1]) for i in range(n_core, n, 2)]
-
-
-def _n_core(spec: "PathSpec", R: int) -> int:
-    return 6 + 6 * R + 6 + (4 if spec.general_attn else 0)
+    stack = param_layout(R, general_attn, add_fc).stack
+    if len(params) != stack.stop:
+        raise _lib.Ta3nError(f"add_fc={add_fc} expects {stack.stop} parameter tensors, got {len(params)}")
+    return [(params[i], params[i + 1]) for i in stack[::2]]
 
 
 def _layer_drop(spec: "PathSpec", layer: int) -> "DropSpec":
@@ -304,15 +329,11 @@ def shared_stack_backward(spec: "PathSpec", xs, xt, w_sh, stack, saved, d_feat, 
 
 
 def _split_params(params, R):
-    it = iter(params)
-    take = lambda n: [next(it) for _ in range(n)]   # noqa: E731
-    shared = take(2)
-    fdisc = take(4)
-    trn_w, trn_b = take(R), take(R)
-    r_w1, r_b1, r_w2, r_b2 = take(R), take(R), take(R), take(R)
-    cls = take(2)
-    vdisc = take(4)
-    return shared, fdisc, trn_w, trn_b, r_w1, r_b1, r_w2, r_b2, cls, vdisc
+    lay = param_layout(R)
+    take = lambda r: [params[i] for i in r]   # noqa: E731
+    rel = lay.rel_disc
+    return (take(lay.shared), take(lay.frame_disc), take(lay.trn_w), take(lay.trn_b),
+            *(take(rel[k * R:(k + 1) * R]) for k in range(4)), take(lay.classifier), take(lay.video_disc))
 
 
 class Buffers:
@@ -356,7 +377,7 @@ def path_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, batch_gemms: boo
     (w_sh, b_sh), (w1f, b1f, w2f, b2f), trn_w, trn_b, r_w1, r_b1, r_w2, r_b2, (w_c, b_c), \
         (w1v, b1v, w2v, b2v) = _split_params(params, R)
     F, H, Cn = w_sh.shape[0], trn_w[0].shape[0], w_c.shape[0]
-    stack = _stack_params(params, _n_core(spec, R), spec.add_fc)
+    stack = _stack_params(params, R, spec.add_fc, spec.general_attn)
     new = bufs.get
     d_v = spec.drop_v.cstruct()
 
@@ -538,9 +559,8 @@ def path_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, bufs: 
         frame_disc_bwd(st, 1)
     stage_done("frame")
     # 1'. shared layers L..1 (layer 1: wgrad only; the input features carry no gradient)
-    n_core = _n_core(spec, R)
-    shared_stack_backward(spec, xs, xt, w_sh, _stack_params(params, n_core, spec.add_fc), saved, d_feat, gin, dw_sh,
-                          db_sh, _stack_params(gout, n_core, spec.add_fc), bufs)
+    shared_stack_backward(spec, xs, xt, w_sh, _stack_params(params, R, spec.add_fc, spec.general_attn), saved, d_feat,
+                          gin, dw_sh, db_sh, _stack_params(gout, R, spec.add_fc, spec.general_attn), bufs)
     stage_done("shared")
 
 
@@ -622,7 +642,7 @@ def avgpool_forward(spec: PathSpec, xs, xt, params, bufs: Buffers, stop_at_video
         raise _lib.Ta3nError("avgpool: the video-level layers must be shared_dim wide (models.py:240-250)")
     new = bufs.get
     d_v = spec.drop_v.cstruct()
-    feats = shared_stack_forward(spec, xs, xt, w_sh, b_sh, _stack_params(params, 12, spec.add_fc), bufs)
+    feats = shared_stack_forward(spec, xs, xt, w_sh, b_sh, _stack_params(params, 0, spec.add_fc), bufs)
     feat = feats[-1]
     hid_f = pred_frame = None
     if spec.use_attn or not stop_at_video_feature:
@@ -698,8 +718,8 @@ def avgpool_backward(spec: PathSpec, dims, xs, xt, params, saved, gin, gout, buf
     check(lib.ta3n_disc_bwd(_p(feat), M * T, F, F, _p(w1f), _p(w2f), _p(hid_f), _p(g_pf), float(spec.beta[2]),
                             _p(d_feat), 1, _p(dw1f), _p(db1f), _p(dw2f), _p(db2f), _p(ws), ws.numel(), st))
     # shared layers L..1
-    shared_stack_backward(spec, xs, xt, w_sh, _stack_params(params, 12, spec.add_fc), saved, d_feat, gin, dw_sh, db_sh,
-                          _stack_params(gout, 12, spec.add_fc), bufs)
+    shared_stack_backward(spec, xs, xt, w_sh, _stack_params(params, 0, spec.add_fc), saved, d_feat, gin, dw_sh, db_sh,
+                          _stack_params(gout, 0, spec.add_fc), bufs)
 
 
 class _AvgPoolPathFunction(torch.autograd.Function):

@@ -37,7 +37,8 @@ from . import loss as LS
 from ._lib import check
 
 _P = TF._p
-_N_LATE = 6     # path_parameters()[0:6] = shared layer W,b + frame discriminator W1,b1,W2,b2: produced last
+_FRAME_LEVEL = TF.param_layout(0)   # the shared layer and the frame discriminator: the same slots at every R
+_N_LATE = _FRAME_LEVEL.frame_disc.stop  # shared layer W,b + frame discriminator W1,b1,W2,b2: produced last
 _ALIGN = 64     # floats: every tensor of a flat buffer starts 256-byte aligned (vector stores, TMA operands)
 _PASS2_KEY = 0x6A09E667F3BCC908     # seed of MCD's second pass = step seed ^ this (its masks differ from pass 1's)
 _STACK_KEY = 0xBB67AE8584CAA73B     # dropout seed of stacked shared layer l (add_fc > 1) = pass seed ^ (l - 1) * this
@@ -143,10 +144,8 @@ def parse_train_stats(words, topk: Sequence[int]) -> TrainStats:
 class TrainStatsSnapshot:
     """``TrainStep.stats_async()``: the accumulator copied to pinned host memory behind an event."""
 
-    def __init__(self, host: torch.Tensor, event, topk: Tuple[int, ...], dis_host: Optional[torch.Tensor] = None,
-                 ent_host: Optional[torch.Tensor] = None, prec_host: Optional[torch.Tensor] = None):
-        self._host, self._event, self._topk, self._dis_host, self._ent_host = host, event, topk, dis_host, ent_host
-        self._prec_host = prec_host
+    def __init__(self, host: torch.Tensor, event, topk: Tuple[int, ...], extra=()):
+        self._host, self._event, self._topk, self._extra = host, event, topk, extra
 
     def done(self) -> bool:
         return self._event.query()
@@ -155,12 +154,8 @@ class TrainStatsSnapshot:
         """Wait for the copy (not for later work on the stream) and return the snapshot."""
         self._event.synchronize()
         st = parse_train_stats(self._host.numpy(), self._topk)
-        if self._dis_host is not None:
-            st.loss_d = dis_meter(self._dis_host.numpy())
-        if self._ent_host is not None:
-            st.loss_e = dis_meter(self._ent_host.numpy())
-        if self._prec_host is not None:
-            sv_prec(st, self._prec_host.numpy())
+        for host, fold in self._extra:
+            fold(st, host.numpy())
         return st
 
 
@@ -180,6 +175,14 @@ def dis_meter(words) -> Meter:
     {sum of val * n, last val, sum of n} (3 doubles)."""
     s, val, n = (float(x) for x in words)
     return Meter(val=val, avg=s / n if n else 0.0, sum=s, count=int(n))
+
+
+def _fold_loss_d(st: TrainStats, words) -> None:
+    st.loss_d = dis_meter(words)
+
+
+def _fold_loss_e(st: TrainStats, words) -> None:
+    st.loss_e = dis_meter(words)
 
 
 def lr_dann(lr0: float, p: float) -> float:
@@ -214,11 +217,71 @@ def step_parameters(model):
     return params
 
 
+def param_layout(model) -> TF.ParamLayout:
+    """The index groups of ``step_parameters(model)``."""
+    R = model.train_segments - 1 if model.frame_aggregation == "trn-m" else 0
+    return TF.param_layout(R, model.use_attn == "general", int(getattr(model, "add_fc", 1)),
+                           getattr(model, "ens_DA", "none") == "MCD")
+
+
 def stack_slots(model) -> List[int]:
     """Indices in ``step_parameters(model)`` of the stacked shared layers' tensors (add_fc > 1): W_2, b_2[, W_3, b_3],
     the last entries of ``path_parameters()``."""
-    n_path = len(model.path_parameters())
-    return list(range(n_path - 2 * (int(getattr(model, "add_fc", 1)) - 1), n_path))
+    return list(param_layout(model).stack)
+
+
+def idle_slots(model, flags: int) -> List[int]:
+    """Indices in ``step_parameters(model)`` of the tensors the adaptation loss with ``flags`` (TrainStep.flags:
+    1 relation, 2 video, 4 frame domain CE, 8 attentive entropy) never reaches: the reference leaves their .grad None,
+    and torch.optim then leaves them alone (no weight decay, no momentum; main.py:83)."""
+    lay = param_layout(model)
+    idle = []
+    if not flags & 4 and model.use_attn_frame == "none":
+        idle += lay.frame_disc
+    if not flags & 1 and model.use_attn == "none":
+        idle += lay.rel_disc
+    if not flags & (2 | 8):
+        idle += lay.video_disc
+    return idle
+
+
+def pretrain_slots(model) -> List[int]:
+    """Indices in ``step_parameters(model)`` of P, the tensors the source-only class loss reaches: all but the video
+    discriminator, the relation discriminators unless the attention weights read them, and the frame discriminator
+    unless the frame attention reads it."""
+    lay = param_layout(model)
+    outside = set(lay.video_disc)
+    if model.use_attn == "none":
+        outside |= set(lay.rel_disc)
+    if model.use_attn_frame == "none":
+        outside |= set(lay.frame_disc)
+    return [i for i in range(lay.head2.stop) if i not in outside]
+
+
+def _padded(numel: int) -> int:
+    """The floats a tensor of ``numel`` floats takes in a flat buffer."""
+    return -(-numel // _ALIGN) * _ALIGN
+
+
+def slot_ranges(params, offs, slots) -> List[Tuple[int, int]]:
+    """The element ranges [lo, hi) of the flat-buffer slots ``slots`` (indices into ``params``, at the offsets ``offs``
+    of ``bucket_layout``), padding included, in buffer order with adjacent ones merged."""
+    ranges = []
+    for i in sorted(slots, key=lambda i: offs[i]):
+        lo, hi = offs[i], offs[i] + _padded(params[i].numel())
+        if ranges and ranges[-1][1] == lo:
+            ranges[-1] = (ranges[-1][0], hi)
+        else:
+            ranges.append((lo, hi))
+    return ranges
+
+
+def _mask_without(like: torch.Tensor, ranges) -> torch.Tensor:
+    """Ones shaped as ``like``, zero over ``ranges``."""
+    mask = torch.ones_like(like)
+    for lo, hi in ranges:
+        mask[lo:hi] = 0.0
+    return mask
 
 
 def bucket_layout(params, stack: Sequence[int] = ()):
@@ -229,15 +292,16 @@ def bucket_layout(params, stack: Sequence[int] = ()):
     Returns (order, offsets-by-index, total, early_total)."""
     stack = list(stack)
     early_order = [i for i in range(_N_LATE, len(params)) if i not in stack]
+    shared, frame_disc = list(_FRAME_LEVEL.shared), list(_FRAME_LEVEL.frame_disc)
     if stack:
         pairs = [stack[i:i + 2] for i in range(0, len(stack), 2)]
-        late = list(range(2, _N_LATE)) + [i for pair in reversed(pairs) for i in pair] + [0, 1]
+        late = frame_disc + [i for pair in reversed(pairs) for i in pair] + shared
     else:
-        late = list(range(_N_LATE))
+        late = shared + frame_disc
     offs, off, early = {}, 0, 0
     for idx in early_order + late:
         offs[idx] = off
-        off += -(-params[idx].numel() // _ALIGN) * _ALIGN
+        off += _padded(params[idx].numel())
         if idx == early_order[-1]:
             early = off
     return early_order + late, offs, off, early
@@ -418,6 +482,73 @@ def optimizer_state_from_torch(model, opt: Optimizer, sd: dict, flat_state: Dict
     return float(grp["lr"]), step
 
 
+def _resolve_mode(model, mode, beta, class_weight, domain_weight, world, *, sampler, stats, use_target, dis_DA,
+                  add_loss_DA, pretrain_source, overlap) -> str:
+    """The executor TrainStep runs (``mode``, else TA3N_STEP_MODE, else the default), after the rules on which options
+    need which executor and which run on a single rank.  Host-only: runs before anything is allocated."""
+    env = os.environ.get("TA3N_STEP_MODE")
+    # class / domain weights and the DANN beta schedule: carried by the step program only
+    step_only = class_weight is not None or any(float(b) < 0 for b in beta) or \
+        tuple(float(w) for w in domain_weight) != (1.0, 1.0)
+    # the features the per-operator sequence has and the step program does not; refused rather than run on another
+    # executor (a value outside an option's set is refused by that option's own check)
+    legacy_only = [(f"use_target={use_target!r}", use_target in ("Sv", "none"), "the unsupervised loss only"),
+                   ("add_fc > 1", int(getattr(model, "add_fc", 1)) > 1, "one shared layer"),
+                   ("ens_DA='MCD'", getattr(model, "ens_DA", "none") == "MCD", "one pass"),
+                   ("add_loss_DA='target_entropy'", add_loss_DA == "target_entropy", "no target-entropy term"),
+                   ("dis_DA", dis_DA in ("DAN", "JAN"), "no discrepancy loss"),
+                   ("pretrain_source", bool(pretrain_source), "one update per iteration")]
+    for name, on, lacks in legacy_only:
+        if not on:
+            continue
+        if (mode or (env if env is not None else "legacy")) != "legacy":
+            raise NotImplementedError(f"{name} runs in mode='legacy' only (the step program has {lacks})")
+        if step_only:
+            raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
+                                      f"(mode='phased'), which does not cover {name}")
+        mode = "legacy"
+    if world > 1:
+        single_rank = [
+            # a short last global batch needs a rule for weighting the ranks' means, and a rank may get no real row
+            (sampler is not None, "the device sampler feeds a single rank; with several ranks use "
+                                  "PairedFeatureLoader + load() / prefetch()"),
+            # each rank would fold its own shard; the global meters need the per-level sums combined every step
+            (stats, "stats=True keeps the meters of a single rank; with several ranks they would have to be combined "
+                    "across ranks every step"),
+            # the target labels (Sv) would have to be sharded with the target rows
+            (use_target in ("Sv", "none"), f"use_target={use_target!r} runs on a single rank"),
+            # every row is paired with every other row of the batch: an MMD per shard is a different loss
+            (dis_DA in ("DAN", "JAN"), "dis_DA runs on a single rank: the MMD pairs rows across the whole batch"),
+            # the pre-training update would need an all-reduce of its own before it is applied, and the peer
+            # all-reduce takes the step counter as a once-per-step sequence number
+            (pretrain_source, "pretrain_source runs on a single rank")]
+        for on, why in single_rank:
+            if on:
+                raise NotImplementedError(why)
+    if mode is None:
+        # 'legacy' (the per-operator sequence) is the fastest executor measured so far and honours the selected GEMM
+        # engine (DESIGN 4.4); the features only the step program has select 'phased', which honours the engine too
+        mode = "phased" if (step_only and model.use_attn_frame == "none") else "legacy"
+        mode = env if env is not None else mode
+    if mode not in ("phased", "legacy"):
+        raise ValueError(f"unknown TrainStep mode {mode!r}")
+    if mode != "legacy" and model.use_attn_frame != "none":
+        raise NotImplementedError("the step program does not cover use_attn_frame; use mode='legacy'")
+    if mode != "legacy" and any(overlap):
+        raise ValueError("overlap_wgrad / parallel_branches / overlap_allreduce / graph_collectives are options "
+                         "of mode='legacy' (the step program runs its launches on one stream)")
+    if mode == "legacy":
+        if any(float(b) < 0 for b in beta):
+            raise ValueError("negative beta (= DANN schedule, main.py:350-352) needs mode='phased': the "
+                             "legacy sequence bakes beta into the captured graph")
+        if class_weight is not None:
+            raise ValueError("class_weight needs mode='phased'")
+        # the per-operator loss kernel has no domain weights
+        if tuple(float(w) for w in domain_weight) != (1.0, 1.0):
+            raise ValueError("domain_weight needs mode='phased'")
+    return mode
+
+
 class TrainStep:
     """Options ``overlap_wgrad`` / ``parallel_branches`` put independent parts of the backward on forked streams
     inside the captured graph.  Forked sub-wave tensor-core GEMM nodes of one graph were found not to overlap under
@@ -440,13 +571,17 @@ class TrainStep:
         supports use_attn_frame); 'phased' = the step program as 14 launches (ta3n_step_run_phased; default when class /
         domain weights or a scheduled beta are given).  class_weight / domain_weight: the weights of criterion /
         criterion_domain (main.py:160-167, 204-205; phased mode).  A negative beta entry selects the DANN schedule for
-        that level (main.py:350-352): call set_progress(p) every step.
+        that level (main.py:350-352): call set_progress(p) every step.  Weights or a negative beta under mode 'legacy'
+        raise ValueError.
+        ens_DA='MCD', add_fc > 1, use_target 'Sv' / 'none', add_loss_DA='target_entropy', dis_DA and pretrain_source
+        ("legacy only" below) run in mode 'legacy' only: with any of them, mode='phased' raises NotImplementedError,
+        and so do class / domain weights and a negative beta (which only the step program has).
         allreduce (world > 1): 'peer' = this library's one-kernel all-reduce over NVLink peer / NVSwitch multicast
         memory (csrc/allreduce.cuh; the gradient bucket then lives in symmetric memory and the whole iteration --
         step, all-reduce, optimizer -- is one CUDA graph), 'nccl' = torch.distributed all_reduce between graphs;
         default: 'peer' when symmetric memory can be set up (and no NCCL overlap option was asked for), else 'nccl'.
 
-        ens_DA='MCD' (mode 'legacy' only): the iteration of main.py:418-583 with --ens_DA MCD is two passes, both in
+        ens_DA='MCD' (legacy only): the iteration of main.py:418-583 with --ens_DA MCD is two passes, both in
         the one graph.  Pass 1 (reverse=False) is the step above plus the second classifier on the source rows and its
         class CE (main.py:447-448).  Pass 2 (reverse=True) runs the target rows only, with their own dropout masks
         (pass2_seeds), for -dis_MCD(out_t, out_t_2) (main.py:548-556, loss.py:29-30); its target logits of the first
@@ -472,7 +607,7 @@ class TrainStep:
         ``stats_topk`` (one to four k in [1, C]) on the batch's real source rows.  ``stats()`` reads them back,
         ``stats_async()`` without stalling the stream, ``reset_stats()`` starts an epoch.  Single rank only.
 
-        dis_DA ('DAN' / 'JAN', mode 'legacy', single rank): the discrepancy loss of main.py:455-505 on this pass's
+        dis_DA ('DAN' / 'JAN', legacy only, single rank): the discrepancy loss of main.py:455-505 on this pass's
         video logits (after dropout_v) and video feature (before it), added to the loss as alpha * loss_d
         (``loss.discrepancy_loss``; three launches after the loss launches, ``ta3n_discrepancy_fwd_bwd``).  DAN takes
         the levels l with place_dis[l] == 'Y' (0: logits, 1: video feature; the 3-D shared-layer levels are refused, as
@@ -484,15 +619,13 @@ class TrainStep:
         With stats=True the ``loss`` meter includes alpha * loss_d and ``TrainStats.loss_d`` holds the term.
 
         add_loss_DA: 'attentive_entropy' (main.py:559-562; needs use_attn and place_adv[0] == place_adv[1] == 'Y' to
-        act), 'target_entropy' or 'none'; any other value raises ValueError.  'target_entropy' (mode 'legacy'; class /
-        domain weights and a negative beta are refused) adds gamma * the mean entropy of softmax over the real target
+        act), 'target_entropy' or 'none'; any other value raises ValueError.  'target_entropy' (legacy only) adds gamma * the mean entropy of softmax over the real target
         rows' class logits (main.py:541-545, loss.py:8-12), one launch after the loss launches
         (``ta3n_target_entropy_fwd_bwd``); a batch with no real target row contributes 0.  Under MCD it reads pass 1's
         target logits (main.py:542 runs before the reverse pass).  With stats=True the ``loss`` meter includes gamma *
         the term and ``TrainStats.loss_e`` holds the term, n = the real target rows (main.py:544).
 
-        pretrain_source (mode 'legacy', single rank, needs an optimizer; class / domain weights and a negative beta are
-        refused): main.py:388-414 with --pretrain_source, in the same graph ahead of the adaptation pass.  A forward of
+        pretrain_source (legacy only, single rank, needs an optimizer): main.py:388-414 with --pretrain_source, in the same graph ahead of the adaptation pass.  A forward of
         the source rows only, with dropout masks of its own, CE(out_s) (+ CE(out_s_2) under MCD), its backward into the
         gradient bucket, clip_grad_norm_ and the optimizer over the parameters that loss reaches (P: the shared layers,
         the TRN, the classifier(s), the relation discriminators under use_attn and the frame discriminator under frame
@@ -501,12 +634,12 @@ class TrainStep:
         counts two steps per iteration for P's parameters and one for the others, as torch.optim.Adam does.
 
         use_target: what the target domain is used for (main.py --use_target).  'uSv' (default): unsupervised
-        adaptation, the iteration above.  'Sv' (mode 'legacy', single rank; class / domain weights and a negative beta
-        are refused; ens_DA='MCD' raises NotImplementedError, as main.py:448 then fails): the class CE runs over the
+        adaptation, the iteration above.  'Sv' (legacy only, single rank; ens_DA='MCD' raises NotImplementedError, as
+        main.py:448 then fails): the class CE runs over the
         real source AND target rows with the target labels (main.py:442-446; ``ta3n_loss_fwd_bwd_sv``), every DA term
         as configured.  ``load`` / ``prefetch`` / ``__call__`` then need ``target_labels`` and a device sampler also
         gathers them.  With stats=True, loss_c and top-k are main.py's: over the source and target rows, n = the real
-        source rows (``ta3n_train_stats_accumulate_sv``).  'none' (same refusals; a model with ens_DA='MCD' raises
+        source rows (``ta3n_train_stats_accumulate_sv``).  'none' (legacy only, single rank; a model with ens_DA='MCD' raises
         ValueError, as main.py:74 never builds one): the source-only baseline.  The iteration is the source pass of
         pretrain_source with the step's own dropout masks -- forward of the source rows, CE (main.py:446), backward,
         clip and the optimizer over P; the other parameters' gradient slots stay zero and they get no update (two
@@ -525,17 +658,10 @@ class TrainStep:
         if sampler is not None:
             if double_buffer:
                 raise ValueError("double_buffer overlaps host-to-device copies; with a device sampler there are none")
-            if (dist.get_world_size(process_group) if dist.is_initialized() else 1) > 1:
-                # a short last global batch needs a rule for weighting the ranks' means, and a rank may get no real row
-                raise NotImplementedError("the device sampler feeds a single rank; with several ranks use "
-                                          "PairedFeatureLoader + load() / prefetch()")
             if (int(sampler.batch[0]), int(sampler.batch[1])) != (int(batch_source), int(batch_target)):
                 raise ValueError(f"sampler batches {sampler.batch} != TrainStep({batch_source}, {batch_target})")
-        if stats and (dist.get_world_size(process_group) if dist.is_initialized() else 1) > 1:
-            # each rank would fold its own shard; the global meters need the per-level sums combined every step
-            raise NotImplementedError("stats=True keeps the meters of a single rank; with several ranks they would "
-                                      "have to be combined across ranks every step")
         self.sampler = sampler
+        self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
         ens = getattr(model, "ens_DA", "none")
         if model.use_attn == "general" or ens not in ("none", "MCD") or model.frame_aggregation != "trn-m":
             # the off-path variants (SURVEY 8f n4) run through VideoModel.forward + autograd; the captured step covers
@@ -546,86 +672,45 @@ class TrainStep:
         if use_target not in ("uSv", "Sv", "none"):
             raise ValueError(f"use_target must be 'uSv', 'Sv' or 'none', got {use_target!r}")
         self.use_target = use_target
-        if use_target != "uSv":
-            if ens == "MCD":
-                if use_target == "none":
-                    raise ValueError("use_target='none' with ens_DA='MCD': main.py:74 builds the source-only model "
-                                     "without MCD; build VideoModel(..., ens_DA='none')")
-                raise NotImplementedError("use_target='Sv' with ens_DA='MCD': main.py:448 applies the second "
-                                          "classifier's source logits to the source and target labels and fails")
-            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
-                raise NotImplementedError(f"use_target={use_target!r} runs in mode='legacy' only (the step program "
-                                          "has the unsupervised loss only)")
-            if class_weight is not None or any(float(b) < 0 for b in beta) or \
-                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
-                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
-                                          f"(mode='phased'), which does not cover use_target={use_target!r}")
-            if (dist.get_world_size(process_group) if dist.is_initialized() else 1) > 1:
-                # the target labels (Sv) would have to be sharded with the target rows
-                raise NotImplementedError(f"use_target={use_target!r} runs on a single rank")
-            mode = "legacy"
+        if use_target != "uSv" and ens == "MCD":
             if use_target == "none":
-                # main.py guards every DA term with use_target != 'none' (:455, :508, :542, :548, :559)
-                place_adv, add_loss_DA, dis_DA, alpha = ("N", "N", "N"), "none", "none", 0.0
+                raise ValueError("use_target='none' with ens_DA='MCD': main.py:74 builds the source-only model "
+                                 "without MCD; build VideoModel(..., ens_DA='none')")
+            raise NotImplementedError("use_target='Sv' with ens_DA='MCD': main.py:448 applies the second "
+                                      "classifier's source logits to the source and target labels and fails")
+        mode = _resolve_mode(model, mode, beta, class_weight, domain_weight, self.world, sampler=sampler, stats=stats,
+                             use_target=use_target, dis_DA=dis_DA, add_loss_DA=add_loss_DA,
+                             pretrain_source=pretrain_source,
+                             overlap=(overlap_wgrad, parallel_branches, overlap_allreduce, graph_collectives))
+        if use_target == "none":
+            # main.py guards every DA term with use_target != 'none' (:455, :508, :542, :548, :559)
+            place_adv, add_loss_DA, dis_DA, alpha = ("N", "N", "N"), "none", "none", 0.0
         self.add_fc = int(getattr(model, "add_fc", 1))
-        if self.add_fc > 1:
-            # the step program (phased) and what only it carries -- class / domain weights, the DANN beta schedule --
-            # do not cover the stacked shared layers; refused rather than run on another executor
-            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
-                raise NotImplementedError("add_fc > 1 runs in mode='legacy' only (the step program has one shared "
-                                          "layer)")
-            if class_weight is not None or any(float(b) < 0 for b in beta) or \
-                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
-                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
-                                          "(mode='phased'), which does not cover add_fc > 1")
-            mode = "legacy"
         self.mcd = ens == "MCD"
         self.mu = float(mu)
         if self.mu != 0.0 and not self.mcd:
             raise ValueError("mu scales the gradient of MCD's reverse pass (ens_DA='MCD'); without MCD it does nothing")
-        if self.mcd:
-            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
-                raise NotImplementedError("ens_DA='MCD' runs in mode='legacy' only (the step program has one pass)")
-            if class_weight is not None or any(float(b) < 0 for b in beta) or \
-                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
-                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
-                                          "(mode='phased'), which does not cover ens_DA='MCD'")
-            mode = "legacy"
         if add_loss_DA not in ("none", "attentive_entropy", "target_entropy"):
             raise ValueError(f"add_loss_DA must be 'none', 'attentive_entropy' or 'target_entropy', got {add_loss_DA!r}")
         self.target_entropy = add_loss_DA == "target_entropy"
-        if self.target_entropy:
-            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
-                raise NotImplementedError("add_loss_DA='target_entropy' runs in mode='legacy' only (the step program "
-                                          "has no target-entropy term)")
-            if class_weight is not None or any(float(b) < 0 for b in beta) or \
-                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
-                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
-                                          "(mode='phased'), which does not cover add_loss_DA='target_entropy'")
-            mode = "legacy"
-        if dis_DA != "none":
-            self._check_dis(dis_DA, alpha, mode, class_weight, beta, domain_weight, process_group, place_dis,
-                            batch_source, batch_target)
-            mode = "legacy"
-        elif float(alpha) != 0.0:
+        if dis_DA == "CORAL":
+            raise NotImplementedError("dis_DA='CORAL': main.py:493 calls a CORAL loss that the reference never defines")
+        if dis_DA not in ("none", "DAN", "JAN"):
+            raise ValueError(f"dis_DA must be 'none', 'DAN' or 'JAN', got {dis_DA!r}")
+        if dis_DA == "none" and float(alpha) != 0.0:
             raise ValueError("alpha weights the discrepancy loss (dis_DA='DAN' / 'JAN'); without it it does nothing")
+        if float(alpha) < 0:
+            _negative_alpha(alpha)
+        if dis_DA == "DAN":
+            LS.dis_levels(place_dis, self.add_fc)
+            n = min(int(batch_source), int(batch_target))
+            if n > LS._DIS_CHUNK and n % LS._DIS_CHUNK:
+                raise ValueError(f"dis_DA='DAN' with min(Bs, Bt) = {n}: above 256 rows the reference cuts the batch "
+                                 "into chunks of 256 and fails unless 256 divides it")
         self.pretrain = bool(pretrain_source)
-        if self.pretrain:
-            if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
-                raise NotImplementedError("pretrain_source runs in mode='legacy' only (the step program has one "
-                                          "update per iteration)")
-            if class_weight is not None or any(float(b) < 0 for b in beta) or \
-                    tuple(float(w) for w in domain_weight) != (1.0, 1.0):
-                raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
-                                          "(mode='phased'), which does not cover pretrain_source")
-            if (dist.get_world_size(process_group) if dist.is_initialized() else 1) > 1:
-                # the pre-training update would need an all-reduce of its own before it is applied, and the peer
-                # all-reduce takes the step counter as a once-per-step sequence number
-                raise NotImplementedError("pretrain_source runs on a single rank")
-            if optimizer is None:
-                raise ValueError("pretrain_source is an optimizer step before each adaptation step (main.py:408-414): "
-                                 "it needs TrainStep(optimizer=SGDNesterov(...) or Adam(...))")
-            mode = "legacy"
+        if self.pretrain and optimizer is None:
+            raise ValueError("pretrain_source is an optimizer step before each adaptation step (main.py:408-414): "
+                             "it needs TrainStep(optimizer=SGDNesterov(...) or Adam(...))")
         self.model = model
         self.params = step_parameters(model)
         self.n_path = len(model.path_parameters())     # the path operators' tensors; MCD's second classifier follows
@@ -642,7 +727,6 @@ class TrainStep:
         self.C = model.fc_classifier_video_source.weight.shape[0]
         self.gamma = float(gamma)
         self.group = process_group
-        self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
         self.flags = (1 if place_adv[0] == "Y" else 0) | (2 if place_adv[1] == "Y" else 0) | \
                      (4 if place_adv[2] == "Y" else 0)
         if add_loss_DA == "attentive_entropy" and model.use_attn != "none":
@@ -650,34 +734,14 @@ class TrainStep:
                 # main.py:560 indexes pred_domain_all[1], the video level only when both are on (SURVEY Q8)
                 raise NotImplementedError("attentive_entropy needs place_adv[0] == place_adv[1] == 'Y'")
             self.flags |= 8
-        # split the step in two graphs around the first gradient bucket only when there is something to overlap
-        if mode is None:
-            # 'legacy' (the per-operator sequence) is the fastest executor measured so far and honours the selected
-            # GEMM engine (DESIGN 4.4); the features only the step program has (class / domain weights, the DANN beta
-            # schedule) select 'phased', which honours the engine too.
-            needs_step = class_weight is not None or any(float(b) < 0 for b in beta) or \
-                tuple(float(w) for w in domain_weight) != (1.0, 1.0)
-            mode = "phased" if (needs_step and model.use_attn_frame == "none") else "legacy"
-            mode = os.environ.get("TA3N_STEP_MODE", mode)
-        if mode not in ("phased", "legacy"):
-            raise ValueError(f"unknown TrainStep mode {mode!r}")
-        if mode != "legacy" and model.use_attn_frame != "none":
-            raise NotImplementedError("the step program does not cover use_attn_frame; use mode='legacy'")
         if overlap_wgrad is None:
             # measured at cfg2 (tools/legacy_options.py): the weight-gradient launches on a forked stream of the graph
             # gain 12 us per step under the tf32x3 engine (its small precise launch overlaps the data-gradient chain)
             # and lose 16 us under plain tf32
             overlap_wgrad = mode == "legacy" and _lib.get_gemm_engine() == "tf32x3" and not overlap_allreduce
-        if mode != "legacy" and (overlap_wgrad or parallel_branches or overlap_allreduce or graph_collectives):
-            raise ValueError("overlap_wgrad / parallel_branches / overlap_allreduce / graph_collectives are options "
-                             "of mode='legacy' (the step program runs its launches on one stream)")
         self.mode = mode
         self.beta_spec = [float(b) for b in beta]
-        if mode == "legacy" and any(b < 0 for b in self.beta_spec):
-            raise ValueError("negative beta (= DANN schedule, main.py:350-352) needs mode='phased': the "
-                             "legacy sequence bakes beta into the captured graph")
-        if class_weight is not None and mode == "legacy":
-            raise ValueError("class_weight needs mode='phased'")
+        # split the step in two graphs around the first gradient bucket only when there is something to overlap
         self._overlap_requested = bool(overlap_allreduce)
         self.split = (self.world > 1) if overlap_allreduce is None else bool(overlap_allreduce)
         if model.use_attn_frame != "none" or mode != "legacy" or self.mcd or use_target == "none":
@@ -725,22 +789,10 @@ class TrainStep:
             self.grad_stats = torch.zeros(2, device=dev, dtype=torch.float32)     # [total_norm, clip_coef]
             # zero-initialised: the Adam kernel's arrival counter starts (and stays, between launches) at 0
             self.opt_ws = torch.zeros(max(1, ws_bytes // 4), device=dev, dtype=torch.float32)
-            # parameters the configured losses never reach keep grad = None in the reference, and torch.optim.SGD then
-            # leaves them alone (no weight decay, no momentum; main.py:83): mask their slots out of the fused update
-            R = self.R
-            idle = []
-            if not (self.flags & 4) and model.use_attn_frame == "none":
-                idle += [2, 3, 4, 5]                                  # frame discriminator
-            if not (self.flags & 1) and model.use_attn == "none":
-                idle += list(range(6 + 2 * R, 6 + 6 * R))             # relation discriminators
-            if not (self.flags & 2) and not (self.flags & 8):
-                n_core = 6 + 6 * R + 6
-                idle += list(range(n_core - 4, n_core))                         # video discriminator
-            self.active_mask = None
+            # the parameters the configured losses never reach are masked out of the fused update
+            idle = idle_slots(model, self.flags)
             if idle:
-                self.active_mask = torch.ones_like(self.flat_grad)
-                for idx in idle:
-                    self.active_mask[offs[idx]:offs[idx] + -(-self.params[idx].numel() // _ALIGN) * _ALIGN] = 0.0
+                self.active_mask = _mask_without(self.flat_grad, slot_ranges(self.params, offs, idle))
 
         f32 = dict(device=dev, dtype=torch.float32)
         # input slots: one, or two for prefetching the next mini-batch while this one computes
@@ -771,7 +823,6 @@ class TrainStep:
         self.bufs = TF.Buffers(dev, persistent=True)
         self.loss_ws = self.bufs.workspace("loss", _lib.load().ta3n_loss_workspace_bytes(self.M))
 
-        di, dv = float(model.dropout_rate_i), float(model.dropout_rate_v)
         # independent dropout masks per data-parallel rank, like the reference's DataParallel replicas
         rank = dist.get_rank(process_group) if dist.is_initialized() else 0
         seed = (int(seed) ^ (rank * 0x9E3779B97F4A7C15)) & (2 ** 63 - 1)
@@ -783,19 +834,14 @@ class TrainStep:
         if self.class_weight is not None and self.class_weight.numel() != self.C:
             raise ValueError("class_weight must have one entry per class")
         self.domain_weight = (float(domain_weight[0]), float(domain_weight[1]))
-        self.spec = TF.PathSpec(
-            num_segments=self.T, beta=tuple(max(b, 0.0) for b in self.beta_spec), mu=0.0, reverse=False,
-            use_attn=model.use_attn != "none", use_attn_frame=model.use_attn_frame != "none",
-            drop_i=TF.DropSpec(p=di, seed=seed, step=self.step_counter) if di > 0 else TF.DropSpec(),
-            drop_v=TF.DropSpec(p=dv, seed=seed ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec(),
-            add_fc=self.add_fc, drop_stack=self._stack_drops(seed, di))
+        self.spec = self._pass_spec(seed)
         if self.mcd:
-            self._init_mcd(seed, di, dv, offs)
+            self._init_mcd(seed, offs)
         if self.pretrain or use_target == "none":
-            self._init_pretrain(seed, di, dv, offs)
+            self._init_pretrain(seed, offs)
         if use_target == "none":
             # the iteration is the source pass with the step's own masks; its update covers P only
-            self.spec_src = self._source_spec(seed, di, dv)
+            self.spec_src = self._pass_spec(seed, classify_only=True)
             self.active_mask = self.pretrain_mask if optimizer is not None else None
         self._init_stats(stats, stats_topk)
         self._init_dis(dis_DA, alpha, place_dis)
@@ -803,6 +849,9 @@ class TrainStep:
             self.pred_video_t1 = torch.zeros(self.Bt, self.C, **f32)
         self.ent_meter = torch.zeros(3, device=dev, dtype=torch.float64) \
             if (self.target_entropy and self.keep_stats) else None
+        # the meters kept beside the accumulator by launches of their own, and how each folds into TrainStats
+        meters = ((self.dis_meter, _fold_loss_d), (self.ent_meter, _fold_loss_e), (self.prec_sum, sv_prec))
+        self._extra_meters = [(acc, fold) for acc, fold in meters if acc is not None]
         self.outputs = None
         self.branch_stream = torch.cuda.Stream(device=dev) if parallel_branches else None
         self.overlap_wgrad = bool(overlap_wgrad)
@@ -828,35 +877,11 @@ class TrainStep:
         if self.keep_stats:
             self.reset_stats()      # and folded one step into the meters
 
-    def _check_dis(self, dis_DA, alpha, mode, class_weight, beta, domain_weight, group, place_dis, Bs, Bt):
-        """The options dis_DA cannot run with (raised at construction, before anything is allocated)."""
-        if dis_DA == "CORAL":
-            raise NotImplementedError("dis_DA='CORAL': main.py:493 calls a CORAL loss that the reference never defines")
-        if dis_DA not in ("DAN", "JAN"):
-            raise ValueError(f"dis_DA must be 'none', 'DAN' or 'JAN', got {dis_DA!r}")
-        if (mode or os.environ.get("TA3N_STEP_MODE", "legacy")) != "legacy":
-            raise NotImplementedError("dis_DA runs in mode='legacy' only (the step program has no discrepancy loss)")
-        if class_weight is not None or any(float(b) < 0 for b in beta) or \
-                tuple(float(w) for w in domain_weight) != (1.0, 1.0):
-            raise NotImplementedError("class / domain weights and the DANN beta schedule need the step program "
-                                      "(mode='phased'), which does not cover dis_DA")
-        if (dist.get_world_size(group) if dist.is_initialized() else 1) > 1:
-            # every row is paired with every other row of the batch: an MMD per shard is a different loss
-            raise NotImplementedError("dis_DA runs on a single rank: the MMD pairs rows across the whole batch")
-        if float(alpha) < 0:
-            _negative_alpha(alpha)
-        if dis_DA == "DAN":
-            LS.dis_levels(place_dis, self.add_fc)
-            n = min(int(Bs), int(Bt))
-            if n > LS._DIS_CHUNK and n % LS._DIS_CHUNK:
-                raise ValueError(f"dis_DA='DAN' with min(Bs, Bt) = {n}: above 256 rows the reference cuts the batch "
-                                 "into chunks of 256 and fails unless 256 divides it")
-
     def _init_dis(self, dis_DA, alpha, place_dis):
         """Buffers of the discrepancy loss: alpha, the unscaled term, the video feature's gradient, the workspace and
         (stats) the loss_d meter; under MCD a copy of pass 1's target logits, which pass 2 overwrites."""
         self.dis_DA = dis_DA
-        self.pred_video_t1 = None
+        self.pred_video_t1 = self.dis_meter = None
         if dis_DA == "none":
             return
         f32 = dict(device=self.device, dtype=torch.float32)
@@ -896,7 +921,7 @@ class TrainStep:
 
     def _init_stats(self, stats, topk):
         """The meters' accumulator (ta3n_train_stats), its workspace and the launch's host arguments."""
-        self.keep_stats = bool(stats)
+        self.keep_stats, self.prec_sum = bool(stats), None
         if not self.keep_stats:
             return
         self.stats_topk = tuple(int(k) for k in topk)
@@ -911,8 +936,7 @@ class TrainStep:
         # backward / the optimizer instead of in front of them (nothing after the loss writes what it reads); a step
         # split in two graphs keeps it on the stream (a branch may not join across graphs)
         self.stats_stream = torch.cuda.Stream(device=self.device) if not self.split else None
-        # the per-operator sequence's loss kernel has no domain weights (the step program applies them)
-        self._stats_dw = (C.c_float * 2)(*(self.domain_weight if self.mode != "legacy" else (1.0, 1.0)))
+        self._stats_dw = (C.c_float * 2)(*self.domain_weight)
         # Sv: the fp64 sums of the top-k meters (ta3n_train_stats_accumulate_sv)
         self.prec_sum = torch.zeros(4, device=self.device, dtype=torch.float64) if self.use_target == "Sv" else None
 
@@ -952,12 +976,8 @@ class TrainStep:
         """The meters since the last ``reset_stats()`` (one blocking readback on the current stream)."""
         self._need_stats("stats")
         st = parse_train_stats(self.stats_acc.cpu().numpy(), self.stats_topk)
-        if self.dis_DA != "none":
-            st.loss_d = dis_meter(self.dis_meter.cpu().numpy())
-        if self.ent_meter is not None:
-            st.loss_e = dis_meter(self.ent_meter.cpu().numpy())
-        if self.prec_sum is not None:
-            sv_prec(st, self.prec_sum.cpu().numpy())
+        for acc, fold in self._extra_meters:
+            fold(st, acc.cpu().numpy())
         return st
 
     def stats_async(self) -> TrainStatsSnapshot:
@@ -966,42 +986,35 @@ class TrainStep:
         self._need_stats("stats_async")
         host = torch.empty(_STATS_WORDS, dtype=torch.int64, pin_memory=True)
         host.copy_(self.stats_acc, non_blocking=True)
-        dis_host = None
-        if self.dis_DA != "none":
-            dis_host = torch.empty(3, dtype=torch.float64, pin_memory=True)
-            dis_host.copy_(self.dis_meter, non_blocking=True)
-        ent_host = None
-        if self.ent_meter is not None:
-            ent_host = torch.empty(3, dtype=torch.float64, pin_memory=True)
-            ent_host.copy_(self.ent_meter, non_blocking=True)
-        prec_host = None
-        if self.prec_sum is not None:
-            prec_host = torch.empty(4, dtype=torch.float64, pin_memory=True)
-            prec_host.copy_(self.prec_sum, non_blocking=True)
+        extra = []
+        for acc, fold in self._extra_meters:
+            extra.append((torch.empty(acc.shape, dtype=acc.dtype, pin_memory=True), fold))
+            extra[-1][0].copy_(acc, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
-        return TrainStatsSnapshot(host, ev, self.stats_topk, dis_host, ent_host, prec_host)
+        return TrainStatsSnapshot(host, ev, self.stats_topk, extra)
 
     def reset_stats(self) -> None:
         """Start an epoch of meters (main.py builds fresh AverageMeters in every train() call): zeroes the accumulator
         on the current stream, no re-capture."""
         self._need_stats("reset_stats")
         self.stats_acc.zero_()
-        if self.dis_DA != "none":
-            self.dis_meter.zero_()
-        if self.ent_meter is not None:
-            self.ent_meter.zero_()
-        if self.prec_sum is not None:
-            self.prec_sum.zero_()
+        for acc, _ in self._extra_meters:
+            acc.zero_()
 
-    def _stack_drops(self, seed, di):
-        """dropout_i of the stacked shared layers: one seed per layer (``stack_seed``), the step counter as key."""
-        if di <= 0:
-            return ()
-        return tuple(TF.DropSpec(p=di, seed=stack_seed(seed, layer), step=self.step_counter)
-                     for layer in range(2, self.add_fc + 1))
+    def _pass_spec(self, seed, reverse=False, mu=0.0, classify_only=False):
+        """A pass of the path whose dropout masks are keyed by the step counter: dropout_i seeded with ``seed``,
+        dropout_v with seed ^ 0x9E3779B9, the stacked shared layers with ``stack_seed(seed, layer)``."""
+        di, dv = float(self.model.dropout_rate_i), float(self.model.dropout_rate_v)
+        drop = lambda p, s: TF.DropSpec(p=p, seed=s, step=self.step_counter) if p > 0 else TF.DropSpec()  # noqa: E731
+        stack = tuple(drop(di, stack_seed(seed, layer)) for layer in range(2, self.add_fc + 1)) if di > 0 else ()
+        return TF.PathSpec(
+            num_segments=self.T, beta=tuple(max(b, 0.0) for b in self.beta_spec), mu=mu, reverse=reverse,
+            use_attn=self.model.use_attn != "none", use_attn_frame=self.model.use_attn_frame != "none",
+            classify_only=classify_only, drop_i=drop(di, seed), drop_v=drop(dv, seed ^ 0x9E3779B9), add_fc=self.add_fc,
+            drop_stack=stack)
 
-    def _init_mcd(self, seed, di, dv, offs):
+    def _init_mcd(self, seed, offs):
         """State of MCD's second pass: its dropout seeds, buffers, and a second gradient bucket with the bucket's
         layout.  Pass 2 writes its parameter gradients there (every backward entry writes, none accumulates) and one
         elementwise add folds the slots it reached into the bucket: with mu == 0 the two classifiers, which the
@@ -1011,12 +1024,7 @@ class TrainStep:
         M, Bs, Bt, C, H = self.M, self.Bs, self.Bt, self.C, self.model.fc_classifier_video_source.weight.shape[1]
         s2 = (seed ^ _PASS2_KEY) & (2 ** 63 - 1)
         self.pass2_seeds = (s2, s2 ^ 0x9E3779B9)       # (drop_i, drop_v) of pass 2, keyed by the same step counter
-        self.spec2 = TF.PathSpec(
-            num_segments=self.T, beta=self.spec.beta, mu=self.mu, reverse=True, use_attn=self.spec.use_attn,
-            use_attn_frame=self.spec.use_attn_frame, classify_only=True,
-            drop_i=TF.DropSpec(p=di, seed=s2, step=self.step_counter) if di > 0 else TF.DropSpec(),
-            drop_v=TF.DropSpec(p=dv, seed=s2 ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec(),
-            add_fc=self.add_fc, drop_stack=self._stack_drops(s2, di))
+        self.spec2 = self._pass_spec(s2, reverse=True, mu=self.mu, classify_only=True)
         self.bufs2 = TF.Buffers(dev, persistent=True)
         self.x_none = torch.zeros(0, self.T, self.D, **f32)            # pass 2 has no source half
         # pass 2 writes its first classifier's logits over the target rows of pass 1's: those rows of pass 1 feed no
@@ -1029,7 +1037,7 @@ class TrainStep:
         self.g_video_t, self.g_video2_t = torch.zeros(Bt, C, **f32), torch.zeros(Bt, C, **f32)
         self.flat_grad2 = torch.zeros_like(self.flat_grad)
         self.grad_views2 = [self.flat_grad2[offs[i]:offs[i] + p.numel()].view_as(p) for i, p in enumerate(self.params)]
-        cls = 6 + 6 * self.R                         # fc_classifier_video_source.weight (then bias, video disc, head 2)
+        cls = param_layout(self.model).classifier.start      # then its bias, the video disc and head 2
         self.acc_range = (offs[cls], self.early_numel) if self.mu == 0.0 else (0, self.flat_grad.numel())
 
     def _enqueue_mcd_pass2_forward(self, lib, st):
@@ -1066,38 +1074,23 @@ class TrainStep:
         lo, hi = self.acc_range
         check(lib.ta3n_accumulate(_P(self.flat_grad[lo:]), _P(self.flat_grad2[lo:]), hi - lo, st))
 
-    def _init_pretrain(self, seed, di, dv, offs):
+    def _init_pretrain(self, seed, offs):
         """State of the source-only pre-training update: its dropout seeds, buffers, the mask of the parameters its
         loss reaches (P), the bucket ranges outside P and, under Adam, the step count of P's parameters."""
         dev, f32 = self.device, dict(device=self.device, dtype=torch.float32)
-        Bs, C, R = self.Bs, self.C, self.R
+        Bs, C = self.Bs, self.C
         s = (seed ^ _PRETRAIN_KEY) & (2 ** 63 - 1)
         self.pretrain_seeds = (s, s ^ 0x9E3779B9)      # (drop_i, drop_v), keyed by the same step counter
-        self.spec_pre = self._source_spec(s, di, dv)
+        self.spec_pre = self._pass_spec(s, classify_only=True)
         self.bufs_pre = TF.Buffers(dev, persistent=True)
         self.x_none = torch.zeros(0, self.T, self.D, **f32)            # the pass has no target half
         self.loss_pre = torch.zeros(1, **f32)
         self.g_video_pre = torch.zeros(Bs, C, **f32)
         if self.mcd:
             self.pred2_pre, self.g_video2_pre = torch.zeros(Bs, C, **f32), torch.zeros(Bs, C, **f32)
-        # P: CE reaches the relation discriminators through the attention weights and the frame discriminator through
-        # the frame attention; it never reaches the video discriminator
-        cls = 6 + 6 * R
-        outside = list(range(cls + 2, cls + 6))
-        if not self.spec.use_attn:
-            outside += list(range(6 + 2 * R, cls))
-        if not self.spec.use_attn_frame:
-            outside += [2, 3, 4, 5]
-        size = lambda i: -(-self.params[i].numel() // _ALIGN) * _ALIGN      # noqa: E731
-        self.pretrain_mask = torch.ones_like(self.flat_grad)
-        ranges = []
-        for i in sorted(outside, key=lambda i: offs[i]):
-            lo, hi = offs[i], offs[i] + size(i)
-            self.pretrain_mask[lo:hi] = 0.0
-            if ranges and ranges[-1][1] == lo:
-                ranges[-1] = (ranges[-1][0], hi)
-            else:
-                ranges.append((lo, hi))
+        outside = set(range(len(self.params))) - set(pretrain_slots(self.model))
+        ranges = slot_ranges(self.params, offs, outside)
+        self.pretrain_mask = _mask_without(self.flat_grad, ranges)
         # the backward does not write these slots, which still hold the previous adaptation pass's gradient: the
         # clip's norm runs over the whole bucket
         self.pretrain_stale = [self.flat_grad[lo:hi] for lo, hi in ranges]
@@ -1108,16 +1101,6 @@ class TrainStep:
         self.pretrain_rest = rest if bool((rest != 0).any()) else None
         if isinstance(self.opt, Adam):
             self.adam_step_pre = torch.zeros(1, device=dev, dtype=torch.int64)
-
-    def _source_spec(self, s, di, dv):
-        """The source-only pass with dropout seeds (s, s ^ 0x9E3779B9) keyed by the step counter: CE on the class
-        logits only, so no video discriminator, and the frame discriminator only under frame attention."""
-        return TF.PathSpec(
-            num_segments=self.T, beta=self.spec.beta, mu=0.0, reverse=False, use_attn=self.spec.use_attn,
-            use_attn_frame=self.spec.use_attn_frame, classify_only=True,
-            drop_i=TF.DropSpec(p=di, seed=s, step=self.step_counter) if di > 0 else TF.DropSpec(),
-            drop_v=TF.DropSpec(p=dv, seed=s ^ 0x9E3779B9, step=self.step_counter) if dv > 0 else TF.DropSpec(),
-            add_fc=self.add_fc, drop_stack=self._stack_drops(s, di))
 
     def _enqueue_pretrain(self, lib, st, optimizer, spec=None, loss=None, after_loss=None):
         """The pre-training update (main.py:388-414): the source rows' forward, CE (+ CE of the second classifier),
@@ -1160,7 +1143,6 @@ class TrainStep:
         """The flat gradient bucket.  With several ranks it is allocated in SYMMETRIC memory (same size on every rank,
         peer-mapped over NVLink, multicast-mapped through the NVSwitch when available) so that the library's own
         all-reduce kernel can read and write every rank's copy (ta3n_allreduce_mean)."""
-        import os
         self.ar = None
         legacy_nccl = self.mode == "legacy" and (self._overlap_requested or self.graph_collectives)
         want = allreduce or os.environ.get("TA3N_ALLREDUCE") or ("nccl" if legacy_nccl else "peer")

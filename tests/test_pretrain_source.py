@@ -11,6 +11,7 @@ iterations against the stock autograd loop with torch.optim; bit-identical eager
 sampler; the meters; the launches the option adds.
 """
 import copy
+import itertools
 import os
 
 import pytest
@@ -80,6 +81,54 @@ def _pretrain_layout(model, idle=()):
             j = [id(q) for q in sp].index(id(p))
             pre[offs[j]:offs[j] + -(-p.numel() // 64) * 64] = 1
     return active, pre, reached
+
+
+def _adaptation_reached(model, place_adv, add_loss_DA):
+    """Names of the parameters that get a gradient in the fp64 oracle's adaptation loss (MCD: both passes)."""
+    cfg = orc.PathConfig(num_class=5, num_segments=5, fc_dim=64, use_attn=model.use_attn,
+                         use_attn_frame=model.use_attn_frame, ens_DA=model.ens_DA)
+    params = {k: v.detach().double() for k, v in model.state_dict().items()}
+    names = orc.used_param_names(params)
+    live = dict(params, **{k: params[k].clone().requires_grad_(True) for k in names})
+    xs, xt = (torch.randn(3, 5, orc.FEATURE_DIM, dtype=torch.float64) for _ in range(2))
+    labels = torch.arange(3)
+    attn = model.use_attn if add_loss_DA == "attentive_entropy" else "none"
+    o1 = orc.forward(live, xs, xt, BETA, 0.0, cfg)
+    if model.ens_DA == "MCD":
+        o2 = mcd.pass2_target(live, xt, BETA, 0.0, cfg)
+        loss = mcd.mcd_loss(o1, o1[2], (o2[1], o2[2]), labels, 0.003, attn, place_adv)
+    else:
+        loss = orc.compose_loss(o1, labels, 0.003, place_adv=place_adv, use_attn=attn)
+    if add_loss_DA == "target_entropy":
+        loss = loss + 0.003 * teo.target_entropy(o1[6])
+    grads = torch.autograd.grad(loss, [live[k] for k in names], allow_unused=True)
+    return {k for k, g in zip(names, grads) if g is not None}
+
+
+@pytest.mark.parametrize("attn,attn_frame", [("TransAttn", "none"), ("none", "none"), ("TransAttn", "TransAttn")])
+@pytest.mark.parametrize("ens", ["none", "MCD"])
+def test_update_set_and_p_are_what_the_oracle_losses_reach(attn, attn_frame, ens):
+    """The slots the fused update keeps (all but ``idle_slots``) are the parameters the fp64 oracle's adaptation loss
+    gives a gradient, for every place_adv and add_loss_DA TrainStep accepts; ``pretrain_slots`` (P) are those its
+    source-only loss gives one."""
+    from ta3n_b200.train import idle_slots, pretrain_slots, step_parameters
+    m = _cpu_model(use_attn=attn, use_attn_frame=attn_frame, ens_DA=ens)
+    sp = step_parameters(m)
+    name = {id(p): k for k, p in m.named_parameters()}
+    slots = lambda names: {j for j, p in enumerate(sp) if name[id(p)] in names}     # noqa: E731
+    for place_adv in itertools.product("YN", repeat=3):
+        for add_loss_DA in ("attentive_entropy", "none", "target_entropy"):
+            entropy = add_loss_DA == "attentive_entropy" and attn != "none"
+            if entropy and place_adv[:2] != ("Y", "Y"):
+                continue        # refused: the attentive entropy reads the video level
+            flags = (place_adv[0] == "Y") | (place_adv[1] == "Y") << 1 | (place_adv[2] == "Y") << 2 | entropy << 3
+            kept = set(range(len(sp))) - set(idle_slots(m, flags))
+            assert kept == slots(_adaptation_reached(m, place_adv, add_loss_DA)), (place_adv, add_loss_DA)
+    cfg = orc.PathConfig(num_class=5, num_segments=5, fc_dim=64, use_attn=attn, use_attn_frame=attn_frame, ens_DA=ens)
+    params = {k: v.detach().double() for k, v in m.state_dict().items()}
+    xs = torch.randn(3, 5, orc.FEATURE_DIM, dtype=torch.float64)
+    _, grads = pto.pretrain_step(params, xs, torch.arange(3), BETA, cfg)
+    assert set(pretrain_slots(m)) == slots({k for k, g in grads.items() if g is not None})
 
 
 @pytest.mark.parametrize("attn,ens", [("TransAttn", "none"), ("none", "none"), ("TransAttn", "MCD")])

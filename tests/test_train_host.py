@@ -1,7 +1,9 @@
 """Host-side logic of ta3n_b200.train that needs no GPU: flat-buffer layout, parameter flattening, schedules."""
+import pytest
 import torch
 
 from oracle import ta3n_oracle as orc
+from ta3n_b200 import Ta3nError
 from ta3n_b200 import train as T
 from ta3n_b200.models import VideoModel
 
@@ -52,6 +54,28 @@ def test_flatten_parameters_preserves_values_names_and_is_idempotent():
     model.load_state_dict(before)
     assert all(p.data_ptr() == flat.data_ptr() + 4 * offs[i] for i, p in enumerate(params))
     assert torch.equal(model.state_dict()["fc_feature_shared_source.weight"], before["fc_feature_shared_source.weight"])
+
+
+@pytest.mark.parametrize("frame_attn,kw,exc,match", [
+    ("TransAttn", dict(mode="phased"), NotImplementedError, "use_attn_frame"),
+    ("none", dict(mode="legacy", class_weight=torch.ones(5)), ValueError, "class_weight needs mode='phased'"),
+    ("none", dict(mode="legacy", beta=(-1.0, 0.6, 0.5)), ValueError, "negative beta"),
+    ("none", dict(mode="legacy", domain_weight=(1.0, 0.5)), ValueError, "domain_weight needs mode='phased'"),
+    # frame attention selects the per-operator sequence, which has no domain weights either
+    ("TransAttn", dict(domain_weight=(1.0, 0.5)), ValueError, "domain_weight needs mode='phased'"),
+])
+def test_executor_refusals_come_before_the_device_check(monkeypatch, frame_attn, kw, exc, match):
+    monkeypatch.delenv("TA3N_STEP_MODE", raising=False)
+    torch.manual_seed(3)
+    m = VideoModel(5, "video", "trn-m", "RGB", train_segments=5, val_segments=5, fc_dim=64, use_attn_frame=frame_attn,
+                   verbose=False).train()
+    kw = dict(dict(beta=(0.75, 0.6, 0.5)), **kw)
+    with pytest.raises(exc, match=match):
+        T.TrainStep(m, 4, 4, **kw)
+    # the step program takes the weights: that configuration passes every check and stops at the device
+    if frame_attn == "none":
+        with pytest.raises(Ta3nError, match="CUDA"):
+            T.TrainStep(m, 4, 4, **dict(kw, mode="phased"))
 
 
 def test_learning_rate_schedule_matches_oracle_restatement_of_main_py():
